@@ -11,7 +11,7 @@ from __future__ import annotations
 import ctypes as C
 from pathlib import Path
 
-AF_ABI_VERSION = 1
+AF_ABI_VERSION = 2
 AF_HIST_BINS = 4096
 AF_HIST_SUB_BITS = 7
 AF_HIST_MIN_EXP = -20
@@ -116,7 +116,7 @@ assert STATS_DTYPE.itemsize == C.sizeof(AfReplicaStats)
 class AfRunPasses(C.Structure):
     _fields_ = [("lane_pass", C.c_int32), ("warp_pass", C.c_int32), ("lane_warps_per_sm", C.c_int32),
                 ("lane_bytes", C.c_int32), ("lane_events_smem", C.c_int32), ("lane_requests_smem", C.c_int32),
-                ("lane_replicas", C.c_uint64), ("warp_replicas", C.c_uint64)]
+                ("lane_replicas", C.c_uint64), ("warp_replicas", C.c_uint64), ("lane_pool_elems", C.c_int32)]
 
 
 class EngineUnavailable(RuntimeError):

@@ -260,13 +260,16 @@ struct af_engine {
     int32_t sweep_cols = 0; uint64_t sweep_rows = 0, sweep_first = 0;
     std::vector<AfSweepColumn> h_sweep_cols;
     std::vector<int32_t> h_sweep_alias;            // aflh::column_aliases of the uploaded values
-    int32_t ev_need = 0;                           // aflh::pending_events_estimate of the scenario + sweep
-    DevBuf d_sweep_cols, d_sweep_vals;
+    int32_t ev_need = 0;                           // aflh::pending_events_estimate of the scenario (replicas without a row)
+    std::vector<int32_t> h_row_need;               // aflh::row_events_estimates of the sweep's rows ...
+    int32_t row_need_max = 0;                      // ... and the largest of them
+    DevBuf d_sweep_cols, d_sweep_vals, d_row_need;
     // thread-per-replica pass: read-only tables (af_lane_host.h), global tiers, the list of flagged replicas
     int mode = AF_MODE_AUTO;
     aflh::Tables lt;
     DevBuf d_l_edges, d_l_servers, d_l_eps, d_l_steps, d_l_spikes, d_l_outages, d_l_lb, d_l_cols, d_gtier, d_redo_list, d_redo_count, d_counter2;
     afl::Cfg C_host{};
+    int32_t last_ev_s = 0, last_rq_s = 0;          // the pool split of the launch's heaviest replica (AfRunPasses)
     bool last_lane = false, last_warp = false; int last_lane_warps = 0;
     // spill + outputs
     DevBuf d_sp_evt, d_sp_evk, d_sp_rq, d_sp_nx;
@@ -345,7 +348,7 @@ void af_engine_destroy(af_engine* e) {
     DevBuf* bufs[] = {&e->d_l_edges, &e->d_l_servers, &e->d_l_eps, &e->d_l_steps, &e->d_l_spikes, &e->d_l_outages, &e->d_l_lb, &e->d_l_cols,
                       &e->d_gtier, &e->d_redo_list, &e->d_redo_count, &e->d_counter2,
                       &e->d_edges, &e->d_servers, &e->d_eps, &e->d_steps, &e->d_lb, &e->d_spikes, &e->d_outages,
-                      &e->d_sweep_cols, &e->d_sweep_vals, &e->d_sp_evt, &e->d_sp_evk, &e->d_sp_rq, &e->d_sp_nx,
+                      &e->d_sweep_cols, &e->d_sweep_vals, &e->d_row_need, &e->d_sp_evt, &e->d_sp_evk, &e->d_sp_rq, &e->d_sp_nx,
                       &e->d_stats, &e->d_sent, &e->d_dropped, &e->d_hist, &e->d_thr, &e->d_ssum, &e->d_smax,
                       &e->d_tclk, &e->d_tser, &e->d_tcnt, &e->d_counter, &e->d_htot};
     for (DevBuf* b : bufs) b->release();
@@ -392,7 +395,7 @@ int af_scenario_upload(af_engine* e, const AfScenario* s) {
     e->sc.outage_marks = e->h_outages.data();
     e->have_scenario = true;
     e->sweep_cols = 0; e->sweep_rows = 0; e->h_sweep_cols.clear();     // a sweep belongs to the scenario it was built for
-    e->ev_need = aflh::pending_events_estimate(e->sc, nullptr);
+    e->ev_need = aflh::pending_events_estimate(e->sc, nullptr); e->row_need_max = 0;
     e->ran = false;
     return AF_OK;
 }
@@ -402,7 +405,7 @@ int af_sweep_upload(af_engine* e, const AfSweep* sw, uint64_t first_replica) {
     if (!e->have_scenario) return e->fail(AF_ERR_STATE, "af_sweep_upload before af_scenario_upload");
     AF_CUDA(e, cudaSetDevice(e->device), "cudaSetDevice");
     AF_CUDA(e, cudaStreamSynchronize(e->stream), "sync before sweep upload");
-    if (!sw || sw->n_columns == 0 || sw->n_rows == 0) { e->sweep_cols = 0; e->sweep_rows = 0; e->h_sweep_cols.clear(); e->ev_need = aflh::pending_events_estimate(e->sc, nullptr); return AF_OK; }
+    if (!sw || sw->n_columns == 0 || sw->n_rows == 0) { e->sweep_cols = 0; e->sweep_rows = 0; e->h_sweep_cols.clear(); e->row_need_max = 0; return AF_OK; }
     if (!sw->columns || !sw->values) return e->fail(AF_ERR_INVALID, "sweep: null columns/values");
     const AfScenario& s = e->sc;
     for (int c = 0; c < sw->n_columns; ++c) {
@@ -439,12 +442,17 @@ int af_sweep_upload(af_engine* e, const AfSweep* sw, uint64_t first_replica) {
         }
     e->h_sweep_cols.assign(sw->columns, sw->columns + sw->n_columns);
     e->h_sweep_alias = aflh::column_aliases(sw->values, sw->n_rows, sw->n_columns);
-    e->ev_need = aflh::pending_events_estimate(e->sc, sw);
+    // each row's own pending-events estimate: the lane kernel splits the replica's shared-memory pool by it.  On the
+    // host, here: one pass over the values (as the checks above), and the kernel's start of a replica stays one load
+    e->row_need_max = aflh::row_events_estimates(e->sc, *sw, e->h_row_need);
     size_t cb = (size_t)sw->n_columns * sizeof(AfSweepColumn), vb = (size_t)sw->n_columns * sw->n_rows * sizeof(double);
     AF_CUDA(e, e->d_sweep_cols.ensure(cb), "sweep columns");
     AF_CUDA(e, e->d_sweep_vals.ensure(vb), "sweep values");
+    AF_CUDA(e, e->d_row_need.ensure(sw->n_rows * sizeof(int32_t)), "sweep row estimates");
     AF_CUDA(e, cudaMemcpyAsync(e->d_sweep_cols.p, sw->columns, cb, cudaMemcpyHostToDevice, e->stream), "sweep columns H2D");
     AF_CUDA(e, cudaMemcpyAsync(e->d_sweep_vals.p, sw->values, vb, cudaMemcpyHostToDevice, e->stream), "sweep values H2D");
+    AF_CUDA(e, cudaMemcpyAsync(e->d_row_need.p, e->h_row_need.data(), sw->n_rows * sizeof(int32_t), cudaMemcpyHostToDevice, e->stream),
+            "sweep row estimates H2D");
     AF_CUDA(e, cudaStreamSynchronize(e->stream), "sweep upload");
     e->sweep_cols = sw->n_columns; e->sweep_rows = sw->n_rows; e->sweep_first = first_replica;
     return AF_OK;
@@ -511,10 +519,20 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
     }
     if (lane) {
         memset(&C, 0, sizeof C);
-        if (!aflh::make_cfg(e->sc, o, e->lt, lane_budget(e, lane_warps), afh::trace_tick_capacity(e->sc), 32, C, getenv("ASYNCFLOW_B200_EVEN_SPLIT") ? 0 : e->ev_need,
-                            getenv("ASYNCFLOW_B200_RQ_MIN") ? atoi(getenv("ASYNCFLOW_B200_RQ_MIN")) : 2)) {     // (experiment knobs)
+        // experiment knobs: every replica on the even split; the record slots the heap leaves
+        const bool even = getenv("ASYNCFLOW_B200_EVEN_SPLIT") != nullptr;
+        if (!aflh::make_cfg(e->sc, o, e->lt, lane_budget(e, lane_warps), afh::trace_tick_capacity(e->sc), 32, C, even ? 0 : e->ev_need,
+                            getenv("ASYNCFLOW_B200_RQ_MIN") ? atoi(getenv("ASYNCFLOW_B200_RQ_MIN")) : 2)) {
             if (e->mode == AF_MODE_LANE) return e->fail(AF_ERR_INVALID, "scenario tables do not fit a lane's shared memory (thread-per-replica engine)");
             lane = false;
+        } else {
+            // the replicas with a sweep row split their pool by the row's estimate, the others by the scenario's
+            const bool rows = !even && e->sweep_cols > 0;
+            const bool all_rows = rows && begin >= e->sweep_first && end - e->sweep_first <= e->sweep_rows;
+            int32_t heaviest = even ? 0 : (rows ? e->row_need_max : e->ev_need);
+            if (rows && !all_rows && e->ev_need > heaviest) heaviest = e->ev_need;
+            aflh::pool_split(C, heaviest, e->last_ev_s, e->last_rq_s);
+            if (rows) { C.need_first = e->sweep_first; C.need_rows = e->sweep_rows; }
         }
     }
     const bool warp = e->mode != AF_MODE_LANE;
@@ -615,6 +633,7 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
         C.spikes = (const afl::SpikeP*)e->d_l_spikes.p; C.outages = (const afl::OutageP*)e->d_l_outages.p;
         C.lb_edges = (const int32_t*)e->d_l_lb.p; C.cols = (const afl::ColP*)e->d_l_cols.p;
         C.sweep_vals = G.sweep_vals; C.sweep_first = G.sweep_first; C.sweep_rows = G.sweep_rows;
+        C.row_need = C.need_rows ? (const int32_t*)e->d_row_need.p : nullptr;
         C.gtier = (unsigned char*)e->d_gtier.p;
         C.stats = G.stats; C.edge_sent = G.edge_sent; C.edge_dropped = G.edge_dropped; C.hist = G.hist; C.thr = G.thr;
         C.samp_sum = G.samp_sum; C.samp_max = G.samp_max; C.trace_clocks = G.trace_clocks; C.trace_series = G.trace_series;
@@ -706,7 +725,8 @@ int af_last_run_passes(af_engine* e, AfRunPasses* out) {
     out->lane_pass = e->last_lane ? 1 : 0; out->warp_pass = e->last_warp ? 1 : 0;
     out->lane_warps_per_sm = e->last_lane_warps;
     out->lane_bytes = e->last_lane ? e->C_host.warp_bytes / 32 : 0;
-    out->lane_events_smem = e->last_lane ? e->C_host.ev_s : 0; out->lane_requests_smem = e->last_lane ? e->C_host.rq_s : 0;
+    out->lane_events_smem = e->last_lane ? e->last_ev_s : 0; out->lane_requests_smem = e->last_lane ? e->last_rq_s : 0;
+    out->lane_pool_elems = e->last_lane ? e->C_host.pool : 0;
     out->lane_replicas = e->last_lane ? e->last_n : 0;
     out->warp_replicas = e->last_warp ? e->last_n : 0;
     if (e->last_lane && e->last_warp) {

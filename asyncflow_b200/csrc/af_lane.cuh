@@ -22,7 +22,9 @@
 // different banks: every access is conflict-free (4 / 2 / 1 wavefronts), no matter how far the replicas have
 // drifted apart.  Tables whose size depends on load (pending events, request records, the now-queue) are TIERED:
 // the first `*_s` entries in shared memory, the rest in a per-lane region of global memory with the same
-// interleave (L2-resident; a branch per access, so that the shared side stays an LDS).  The same region holds the
+// interleave (L2-resident; a branch per access, so that the shared side stays an LDS).  The heap and the request
+// records share ONE pool of 128-bit elements, heap from the bottom, records from the top, split per replica by the
+// replica's own load (pool_events).  The same region holds the
 // cold words (waiter FIFOs, mailboxes, drop counters) and the write-only aggregates (the gauges' sums and
 // maxima, the send counters: fire-and-forget REDs).  Read-only scenario tables are NOT replicated per replica:
 // they are read through the read-only data path (128-bit __ldg) and a swept field is an index into the lane's
@@ -131,25 +133,34 @@ struct Cfg {
     int32_t n_series, n_sweep_cols, n_row;          // n_row: sweep columns kept per lane (looked up during the run)
     int32_t collect_hist, collect_thr, trace_replicas, trace_clock_cap, trace_tick_cap;
     int32_t redo;                                   // 1: replica indices come from redo_list (re-run of flagged replicas)
-    // tiered tables: entries in shared memory / in total
-    int32_t ev_s, ev_total, rq_s, rq_total, nq_s;
-    // shared-memory layout of a warp: 128-bit region (events, then request records), 64-bit region, 32-bit region
-    int32_t o128_ev, o128_rq, n128;
+    // tiered tables: entries in total; the now-queue's entries in shared memory
+    int32_t ev_total, rq_total, nq_s;
+    // The lane's POOL of `pool` 128-bit elements holds the first ev_s heap entries (element i) and the first rq_s request
+    // records (slot s at element pool - 1 - s), ev_s + rq_s = pool, split per replica by pool_events() from the
+    // replica's pending-events estimate row_need[replica - need_first] when the launch has one for the replica; the
+    // others take ev_s / rq_s (make_cfg: the split of the scenario's estimate).  ev_lo: the fewest heap entries a
+    // replica gets, rq_floor: the fewest records when the events take more.
+    int32_t pool, ev_lo, rq_floor, ev_s, rq_s;
+    // shared-memory layout of a warp: 128-bit region (the pool), 64-bit region, 32-bit region
+    int32_t n128;
     int32_t o64_nq, o64_spike, o64_row, n64;
-    int32_t o32_next, o32_conn, o32_srv, o32_lb, o32_dirty, n_dirty, n32;
+    int32_t o32_conn, o32_srv, o32_lb, o32_dirty, n_dirty, n32;
     int32_t warp_bytes;                             // n128 * 512 + n64 * 256 + n32 * 128
-    // global tier of a warp (same interleave).  gi_* = (offset of the table in its region) - (entries kept in shared
-    // memory): entry idx >= split lives at element idx + gi_* of the region
-    int32_t gi_ev, gi_rq, gn128;
+    // global tier of a warp (same interleave).  Heap entry idx >= ev_s at element idx - ev_s of the 128-bit region,
+    // record slot s >= rq_s at element gi_rq + s (= ev_total - ev_s + (s - rq_s): right after the replica's heap entries);
+    // gi_* = (offset of the table in its region) - (entries kept in shared memory)
+    int32_t gi_rq, gn128;
     int32_t gi_nq, gi_acc, gn64;                    // gi_acc: the gauges' accumulators (write-only during the run: RED)
-    int32_t gi_next, g32_cold, gi_smax, gi_sent, gn32;   // ... their maxima, the per-edge send counters (RED too)
+    int32_t g32_cold, gi_smax, gi_sent, gn32;       // words [0, rq_total): every record's `next` link; then the cold words,
+                                                    // the gauges' maxima, the per-edge send counters (RED too)
     int32_t c_srvq, c_inbox, c_drop;                // cold words (offsets from g32_cold): waiter FIFOs, mailboxes, drop counters
     uint64_t gwarp_bytes;                           // gn128 * 512 + gn64 * 256 + gn32 * 128
     // device pointers
     const EdgeP* edges; const ServerP* servers; const EndpointP* endpoints; const StepP* steps;
     const SpikeP* spikes; const OutageP* outages; const int32_t* lb_edges; const ColP* cols;
     const double* sweep_vals; uint64_t sweep_first, sweep_rows;
-    unsigned char* gtier;                           // global tiers, one region per resident warp
+    const int32_t* row_need; uint64_t need_first, need_rows;   // per-replica pending-events estimates (nullptr: ev_s / rq_s for all)
+    unsigned char* gtier;                          // global tiers, one region per resident warp
     AfReplicaStats* stats; uint32_t* edge_sent; uint32_t* edge_dropped;
     uint32_t* hist; uint32_t* thr; uint64_t* samp_sum; uint32_t* samp_max;
     double* trace_clocks; uint32_t* trace_series; uint32_t* trace_counts;
@@ -248,13 +259,6 @@ AFL_IN uint64_t ld_t64(const Mem& m, int32_t os, int32_t gi, int32_t idx, int32_
 AFL_IN void st_t64(const Mem& m, int32_t os, int32_t gi, int32_t idx, int32_t split, uint64_t v) {
     if (AFL_LIKELY(idx < split)) sm_st64(a64(m, os + idx), v); else *g64p(m, gi + idx) = v;
 }
-AFL_IN uint32_t ld_t32(const Mem& m, int32_t os, int32_t gi, int32_t idx, int32_t split) {
-    if (AFL_LIKELY(idx < split)) return sm_ld32(a32(m, os + idx));
-    return *g32p(m, gi + idx);
-}
-AFL_IN void st_t32(const Mem& m, int32_t os, int32_t gi, int32_t idx, int32_t split, uint32_t v) {
-    if (AFL_LIKELY(idx < split)) sm_st32(a32(m, os + idx), v); else *g32p(m, gi + idx) = v;
-}
 
 // the replica's scalar state: registers (nothing here is indexed dynamically)
 struct St {
@@ -263,7 +267,9 @@ struct St {
     uint32_t seq; int32_t ev_n; uint32_t peak_ev;
     uint64_t arr_t; uint32_t arr_seq, arr_on;   // the generator's pending timeout: always exactly one, kept out of the heap
     uint32_t nq_head, nq_tail, busy;            // busy = 2 * (items in the now-queue) + (the heap may hold an event of this instant)
-    uint32_t rq_free, rq_free_hi, rq_hw, rq_live, peak_rq;   // two free lists: slots in shared memory / in the global tier
+    int32_t ev_s, rq_s;                         // this replica's split of the pool: heap entries / record slots in shared memory
+    uint32_t rq_mask;                           // free record slots in shared memory (bit s: slot s < rq_s)
+    uint32_t rq_free_hi, rq_hw, rq_live, peak_rq;   // slots in the global tier: free list, high-water mark (from rq_s)
     uint32_t n_waiting;                         // requests parked in a RAM / CPU waiter FIFO (0: every such FIFO is empty, no need to look)
     double g_vnow, g_wend, g_lam;               // generator: the sampler's virtual clock (the simulation's is `now`)
     uint32_t g_pos, generated, g_done, need_arrival, arm_seq;
@@ -286,29 +292,55 @@ AFL_IN uint32_t ep_total_ram(const Mem& m, uint32_t ep) {
     return p.c_ram >= 0 ? (uint32_t)row_val(m, p.c_ram) : p.total_ram;
 }
 
-// ---- request records (tiered): one 128-bit element  t0 | id : pack  + the `next` link (32-bit table) ------------
+// ---- the pool split (af_lane_host.h reports it for the launch's heaviest replica) -------------------------------
+// Shared-memory record slots are handed out from a 32-bit mask: at most RQ_BITS of them.
+constexpr int32_t RQ_BITS = 32;
+// Heap entries a replica with an estimated `need` pending events keeps in shared memory: its need, but no more than
+// leaves `rq_floor` record slots and no fewer than `ev_lo` (a heap entry is touched ~20 times per event, a record
+// twice: byte for byte the heap is worth more); the records take the rest, at most RQ_BITS and rq_total of them, so
+// the heap takes whatever the records cannot.  make_cfg caps the pool at ev_total + min(rq_total, RQ_BITS): the
+// records always get exactly pool - ev_s slots.
+AFL_IN int32_t pool_events(int32_t pool, int32_t ev_lo, int32_t rq_floor, int32_t ev_total, int32_t rq_total, int32_t need) {
+    int32_t ev = need < pool - rq_floor ? need : pool - rq_floor;
+    if (ev < ev_lo) ev = ev_lo;
+    const int32_t rq_cap = rq_total < RQ_BITS ? rq_total : RQ_BITS;
+    if (ev < pool - rq_cap) ev = pool - rq_cap;
+    return ev < ev_total ? ev : ev_total;
+}
+#if AFL_DEVICE
+AFL_IN uint32_t lowest_bit(uint32_t x) { return (uint32_t)__ffs((int)x) - 1u; }
+#else
+AFL_IN uint32_t lowest_bit(uint32_t x) { return (uint32_t)__builtin_ctz(x); }
+#endif
+
+// ---- request records (tiered): one 128-bit element  t0 | id : pack.  Slot s < rq_s is element pool - 1 - s of the
+//      lane's pool (one LDS.128), the others live in the global tier.  The `next` links (free list of the global slots,
+//      waiter FIFOs) are 32-bit words of the global tier for every slot ------------------------------------------------
 // (Tried in round 2 and dropped: a third tier of 256-record PAGES from a pool shared by all lanes, so that saturated
 //  replicas -- 10^4..10^5 requests parked in a RAM queue -- stay on this engine.  Bit-exact, but the extra tier in every
 //  record access grew the loop's instruction footprint and slowed the bench workload, and C2 (10^4 replicas) was still
 //  faster one replica per warp.)
-AFL_IN void rq_load(const Mem& m, uint32_t s, double& t0, uint32_t& rid, uint32_t& pack) {
+AFL_IN uint32_t rq_sm(const Mem& m, uint32_t s) { return a128(m, AFL_C.pool - 1 - (int32_t)s); }
+AFL_IN unsigned char* rq_gl(const Mem& m, uint32_t s) { return g128p(m, AFL_C.gi_rq + (int32_t)s); }
+AFL_IN void rq_load(const St& W, const Mem& m, uint32_t s, double& t0, uint32_t& rid, uint32_t& pack) {
     uint64_t a, b;
-    ld_t128(m, AFL_C.o128_rq, AFL_C.gi_rq, (int32_t)s, AFL_C.rq_s, a, b);
+    if (AFL_LIKELY((int32_t)s < W.rq_s)) sm_ld128(rq_sm(m, s), a, b); else gl_ld128(rq_gl(m, s), a, b);
     t0 = afr::u2d(a); rid = (uint32_t)b; pack = (uint32_t)(b >> 32);
 }
-AFL_IN void rq_store(const Mem& m, uint32_t s, double t0, uint32_t rid, uint32_t pack) {
-    st_t128(m, AFL_C.o128_rq, AFL_C.gi_rq, (int32_t)s, AFL_C.rq_s, afr::d2u(t0), (uint64_t)rid | ((uint64_t)pack << 32));
+AFL_IN void rq_store(const St& W, const Mem& m, uint32_t s, double t0, uint32_t rid, uint32_t pack) {
+    const uint64_t a = afr::d2u(t0), b = (uint64_t)rid | ((uint64_t)pack << 32);
+    if (AFL_LIKELY((int32_t)s < W.rq_s)) sm_st128(rq_sm(m, s), a, b); else gl_st128(rq_gl(m, s), a, b);
 }
-AFL_IN uint32_t rq_pack(const Mem& m, uint32_t s) {
-    if (AFL_LIKELY((int32_t)s < AFL_C.rq_s)) return sm_ld32(a128(m, AFL_C.o128_rq + (int32_t)s) + 12u);
-    return *reinterpret_cast<const uint32_t*>(g128p(m, AFL_C.gi_rq + (int32_t)s) + 12);
+AFL_IN uint32_t rq_pack(const St& W, const Mem& m, uint32_t s) {
+    if (AFL_LIKELY((int32_t)s < W.rq_s)) return sm_ld32(rq_sm(m, s) + 12u);
+    return *reinterpret_cast<const uint32_t*>(rq_gl(m, s) + 12);
 }
-AFL_IN void rq_pack_set(const Mem& m, uint32_t s, uint32_t v) {
-    if (AFL_LIKELY((int32_t)s < AFL_C.rq_s)) sm_st32(a128(m, AFL_C.o128_rq + (int32_t)s) + 12u, v);
-    else *reinterpret_cast<uint32_t*>(g128p(m, AFL_C.gi_rq + (int32_t)s) + 12) = v;
+AFL_IN void rq_pack_set(const St& W, const Mem& m, uint32_t s, uint32_t v) {
+    if (AFL_LIKELY((int32_t)s < W.rq_s)) sm_st32(rq_sm(m, s) + 12u, v);
+    else *reinterpret_cast<uint32_t*>(rq_gl(m, s) + 12) = v;
 }
-AFL_IN uint32_t rq_next(const Mem& m, uint32_t s) { return ld_t32(m, AFL_C.o32_next, AFL_C.gi_next, (int32_t)s, AFL_C.rq_s); }
-AFL_IN void rq_next_set(const Mem& m, uint32_t s, uint32_t v) { st_t32(m, AFL_C.o32_next, AFL_C.gi_next, (int32_t)s, AFL_C.rq_s, v); }
+AFL_IN uint32_t rq_next(const Mem& m, uint32_t s) { return *g32p(m, (int32_t)s); }
+AFL_IN void rq_next_set(const Mem& m, uint32_t s, uint32_t v) { *g32p(m, (int32_t)s) = v; }
 
 #if AFL_DEVICE
 // fire-and-forget reductions (RED.E.ADD / RED.E.MAX: no result, no scoreboard wait) and the loads that read them back
@@ -326,11 +358,11 @@ static inline uint32_t ld_cg32(const uint32_t* p) { return *p; }
 #endif
 // A request takes the LOWEST tier that has a free slot: with one LIFO list the few requests in flight after a burst
 // keep cycling through whatever slots were freed last -- often global-tier ones (C1 with 10 shared-memory slots for
-// ~3 requests in flight: -9 %).  Shared-memory slots are handed out first (free list, then fresh ones), global ones after.
+// ~3 requests in flight: -9 %).  Shared-memory slots are handed out first (the lowest free bit of the mask), global
+// ones after (free list, then fresh ones).
 AFL_IN uint32_t rq_alloc(St& W, const Mem& m) {
     uint32_t s;
-    if (W.rq_free != NIL) { s = W.rq_free; W.rq_free = rq_next(m, s); }
-    else if ((int32_t)W.rq_hw < AFL_C.rq_s) { s = W.rq_hw++; }
+    if (W.rq_mask != 0u) { s = lowest_bit(W.rq_mask); W.rq_mask &= W.rq_mask - 1u; }
     else if (W.rq_free_hi != NIL) { s = W.rq_free_hi; W.rq_free_hi = rq_next(m, s); }
     else if ((int32_t)W.rq_hw < AFL_C.rq_total) { s = W.rq_hw++; }
     else { W.flags |= AF_FLAG_REQUEST_OVERFLOW; return NIL; }
@@ -339,7 +371,7 @@ AFL_IN uint32_t rq_alloc(St& W, const Mem& m) {
     return s;
 }
 AFL_IN void rq_release(St& W, const Mem& m, uint32_t s) {
-    if ((int32_t)s < AFL_C.rq_s) { rq_next_set(m, s, W.rq_free); W.rq_free = s; }
+    if ((int32_t)s < W.rq_s) W.rq_mask |= 1u << s;
     else { rq_next_set(m, s, W.rq_free_hi); W.rq_free_hi = s; }
     --W.rq_live;
 }
@@ -365,10 +397,11 @@ AFL_COLD uint32_t fifo_pop(const Mem m, int32_t w_head, int32_t w_tail) {
     return s;
 }
 
-// ---- pending timed events: 4-ary min-heap on (time bits, seq), tiered; one 128-bit element per event.  The root is
-//      always in shared memory (make_cfg: ev_s >= 1): the loop reads it with a plain LDS ------------------------------
-AFL_IN void ev_get(const Mem& m, int32_t i, uint64_t& t, uint64_t& k) { ld_t128(m, AFL_C.o128_ev, AFL_C.gi_ev, i, AFL_C.ev_s, t, k); }
-AFL_IN void ev_set(const Mem& m, int32_t i, uint64_t t, uint64_t k) { st_t128(m, AFL_C.o128_ev, AFL_C.gi_ev, i, AFL_C.ev_s, t, k); }
+// ---- pending timed events: 4-ary min-heap on (time bits, seq), tiered; one 128-bit element per event: entry i < ev_s
+//      is element i of the pool.  The root is always in shared memory (pool_events: ev_s >= ev_lo >= 1): the loop reads
+//      it with a plain LDS ---------------------------------------------------------------------------------------------
+AFL_IN void ev_get(const St& W, const Mem& m, int32_t i, uint64_t& t, uint64_t& k) { ld_t128(m, 0, -W.ev_s, i, W.ev_s, t, k); }
+AFL_IN void ev_set(const St& W, const Mem& m, int32_t i, uint64_t t, uint64_t k) { st_t128(m, 0, -W.ev_s, i, W.ev_s, t, k); }
 AFL_IN bool ev_less(uint64_t ta, uint64_t ka, uint64_t tb, uint64_t kb) {       // times are non-negative doubles: bit order = value order
     return ta < tb || (ta == tb && (uint32_t)(ka >> 32) < (uint32_t)(kb >> 32));
 }
@@ -382,12 +415,12 @@ AFL_IN void heap_push(St& W, const Mem& m, uint64_t tb, uint64_t key) {
     while (i > 0) {
         const int32_t p = (i - 1) >> 2;
         uint64_t tp, kp;
-        ev_get(m, p, tp, kp);
+        ev_get(W, m, p, tp, kp);
         if (!ev_less(tb, key, tp, kp)) break;
-        ev_set(m, i, tp, kp);
+        ev_set(W, m, i, tp, kp);
         i = p;
     }
-    ev_set(m, i, tb, key);
+    ev_set(W, m, i, tb, key);
 }
 // remove the root (the caller has read it)
 // One sift-down level = the four children fetched TOGETHER (indices past the end clamped onto the last child: a
@@ -398,7 +431,7 @@ AFL_IN void heap_pop(St& W, const Mem& m) {
     const int32_t n = --W.ev_n;
     if (n == 0) return;
     uint64_t tl, kl;
-    ev_get(m, n, tl, kl);
+    ev_get(W, m, n, tl, kl);
     const int32_t last = n - 1;
     int32_t i = 0;
 #pragma unroll 1
@@ -408,21 +441,21 @@ AFL_IN void heap_pop(St& W, const Mem& m) {
         const int32_t c1 = c + 1 < last ? c + 1 : last, c3 = c + 3 < last ? c + 3 : last;
         int32_t c2 = c + 2 < last ? c + 2 : last;
         uint64_t t0, k0, t1, k1, t2, k2, t3, k3;
-        if (AFL_LIKELY(c3 < AFL_C.ev_s)) {
-            sm_ld128(a128(m, AFL_C.o128_ev + c), t0, k0); sm_ld128(a128(m, AFL_C.o128_ev + c1), t1, k1);
-            sm_ld128(a128(m, AFL_C.o128_ev + c2), t2, k2); sm_ld128(a128(m, AFL_C.o128_ev + c3), t3, k3);
+        if (AFL_LIKELY(c3 < W.ev_s)) {
+            sm_ld128(a128(m, c), t0, k0); sm_ld128(a128(m, c1), t1, k1);
+            sm_ld128(a128(m, c2), t2, k2); sm_ld128(a128(m, c3), t3, k3);
         } else {
-            ev_get(m, c, t0, k0); ev_get(m, c1, t1, k1); ev_get(m, c2, t2, k2); ev_get(m, c3, t3, k3);
+            ev_get(W, m, c, t0, k0); ev_get(W, m, c1, t1, k1); ev_get(W, m, c2, t2, k2); ev_get(W, m, c3, t3, k3);
         }
         int32_t b = c;
         if (ev_less(t1, k1, t0, k0)) { t0 = t1; k0 = k1; b = c1; }
         if (ev_less(t3, k3, t2, k2)) { t2 = t3; k2 = k3; c2 = c3; }
         if (ev_less(t2, k2, t0, k0)) { t0 = t2; k0 = k2; b = c2; }
         if (!ev_less(t0, k0, tl, kl)) break;
-        ev_set(m, i, t0, k0);
+        ev_set(W, m, i, t0, k0);
         i = b;
     }
-    ev_set(m, i, tl, kl);
+    ev_set(W, m, i, tl, kl);
 }
 
 // ---- now-queue (tiered ring of NQ_TOTAL items: seq << 32 | kind:3 aux:9 slot:20) ---------------------
@@ -577,7 +610,7 @@ AFL_IN void ram_walk(St& W, const Mem& m, uint32_t sidx) {
         const uint32_t w = fifo_pop(m, sq_word(sidx, SQ_RAMQ_HEAD), sq_word(sidx, SQ_RAMQ_TAIL));
         W.n_waiting -= 1;
         const uint32_t h = c32_ld(m, sq_word(sidx, SQ_RAMQ_HEAD));
-        if (h != NIL) c32_st(m, sq_word(sidx, SQ_RAMQ_NEED), ep_total_ram(m, pk_ep(rq_pack(m, h))));
+        if (h != NIL) c32_st(m, sq_word(sidx, SQ_RAMQ_NEED), ep_total_ram(m, pk_ep(rq_pack(W, m, h))));
         i32_st(m, sv_word(sidx, SV_RAM_FREE), i32_ld(m, sv_word(sidx, SV_RAM_FREE)) - (int32_t)need);
         nq_push(W, m, I_RAM_OK, sidx, w);
     }
@@ -670,7 +703,14 @@ AFL_IN void start_replica(St& W, const Mem& m, uint64_t local_index) {
     W.now = 0.0; W.horizon = (double)C.horizon_s; W.seq = 0;
     W.ev_n = 0; W.peak_ev = 0; W.arr_t = 0; W.arr_seq = 0; W.arr_on = 0;
     W.nq_head = 0; W.nq_tail = 0; W.busy = 0;
-    W.rq_free = NIL; W.rq_free_hi = NIL; W.rq_hw = 0; W.rq_live = 0; W.peak_rq = 0; W.n_waiting = 0;
+    // this replica's split of the pool, from its own pending-events estimate
+    const uint64_t nr = W.replica - C.need_first;
+    if (C.row_need != nullptr && nr < C.need_rows) {
+        W.ev_s = pool_events(C.pool, C.ev_lo, C.rq_floor, C.ev_total, C.rq_total, C.row_need[nr]);
+        W.rq_s = C.pool - W.ev_s;
+    } else { W.ev_s = C.ev_s; W.rq_s = C.rq_s; }
+    W.rq_mask = W.rq_s >= RQ_BITS ? ~0u : (1u << W.rq_s) - 1u;
+    W.rq_free_hi = NIL; W.rq_hw = (uint32_t)W.rq_s; W.rq_live = 0; W.peak_rq = 0; W.n_waiting = 0;
     W.g_vnow = 0.0; W.g_wend = 0.0; W.g_lam = 0.0; W.g_pos = 0; W.generated = 0; W.g_done = 0;
     W.gap0 = 0.0; W.gap1 = 0.0; W.gap_cnt = 0;
     W.lb_n = C.n_lb_edges; W.spike_cur = 0; W.outage_cur = 0;
@@ -847,7 +887,7 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                 } else {
                     const bool have_heap = W.ev_n > 0, have_ev = have_heap || W.arr_on != 0;
                     uint64_t tb = 0, key = 0;
-                    if (have_heap) sm_ld128(a128(m, AFL_C.o128_ev), tb, key);      // the root is always in shared memory (ev_s >= 1)
+                    if (have_heap) sm_ld128(m.s128, tb, key);      // the root is always in shared memory (ev_s >= 1)
                     const uint64_t root_t = tb;
                     bool take_arr = false;                // the earliest timed event: the heap's root or the generator's timeout
                     if (W.arr_on) {
@@ -866,7 +906,7 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                     if (!is_item && !finish) {
                         bool more;
                         if (take_arr) { W.arr_on = 0u; more = have_heap && root_t == tb; }
-                        else { heap_pop(W, m); more = (W.ev_n > 0 && sm_ld64(a128(m, AFL_C.o128_ev)) == tb) || (W.arr_on && W.arr_t == tb); }
+                        else { heap_pop(W, m); more = (W.ev_n > 0 && sm_ld64(m.s128) == tb) || (W.arr_on && W.arr_t == tb); }
                         W.busy = (W.busy & ~1u) | (more ? 1u : 0u);
                         t_ev = afr::u2d(tb); ev_seq = (uint32_t)(key >> 32); word = (uint32_t)key;
                         is_event = true;
@@ -896,7 +936,7 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
         AFL_TRACE("%s t=%.17g seq=%u kind=%u aux=%u slot=%u\n", is_item ? "it" : "ev", W.now, ev_seq, kind, aux, slot);
         // everything that names a request reads its record here, once, for all kinds
         const bool names_request = is_event ? (kind == K_DELIVER || kind == K_STEP_END) : (is_item && kind != I_CLIENT_LOOP && kind != I_PUT);
-        if (names_request) rq_load(m, slot, t0, rid, pack);
+        if (names_request) rq_load(W, m, slot, t0, rid, pack);
         if (is_event) {
             if (kind == K_DELIVER) {                          // edge.py:110-116: the edge's timeout fired
                 conn_add(W, m, aux, -1);
@@ -906,7 +946,7 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                 node = tk == AF_TARGET_CLIENT ? NODE_CLIENT : (tk == AF_TARGET_LB ? NODE_LB : NODE_SERVER0 + (meta >> 5));
                 if (can_fuse(W)) { act = A_NODE; from_box = false; }   // put -> pending get -> resume, nothing in between
                 else {                                         // (fused implies: every inbox empty, every consumer in get())
-                    rq_pack_set(m, slot, pack);
+                    rq_pack_set(W, m, slot, pack);
                     fifo_push(m, ib_word(node, IB_HEAD), ib_word(node, IB_TAIL), slot);   // Store.put: items.append now ...
                     nq_push(W, m, I_PUT, node, slot);                                       // ... the put event is processed later
                 }
@@ -923,7 +963,7 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                 W.need_arrival = 1;
                 if (slot != NIL) {
                     pack = 1u; edge = (uint32_t)C.gen_edge;        // record_hop(generator)
-                    rq_store(m, slot, W.now, rid, pack);
+                    rq_store(W, m, slot, W.now, rid, pack);
                     act = A_SEND;
                 }
             } else if (kind == K_SPIKE) {
@@ -989,7 +1029,7 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                 if (total_ram) {                               // yield RAM.get(total_ram)
                     if (!(can_fuse(W) && (int32_t)total_ram <= i32_ld(m, sv_word(sidx, SV_RAM_FREE)) && q_empty(W, m, sq_word(sidx, SQ_RAMQ_HEAD)))) {
                         // cannot be served at once: join the queue, walk it
-                        rq_pack_set(m, slot, pack);
+                        rq_pack_set(W, m, slot, pack);
                         if (q_empty(W, m, sq_word(sidx, SQ_RAMQ_HEAD))) c32_st(m, sq_word(sidx, SQ_RAMQ_NEED), total_ram);
                         fifo_push(m, sq_word(sidx, SQ_RAMQ_HEAD), sq_word(sidx, SQ_RAMQ_TAIL), slot);
                         W.n_waiting += 1;
@@ -1017,7 +1057,7 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                     const int32_t lb = C.o32_lb, n = W.lb_n;
                     // every covered server is down: the reference dies here (StopIteration inside round_robin);
                     // the replica stops and says so (flatten() rejects timelines that can reach this state)
-                    if (AFL_UNLIKELY(n <= 0)) { rq_pack_set(m, slot, pack); W.flags |= AF_FLAG_LB_EMPTY; }
+                    if (AFL_UNLIKELY(n <= 0)) { rq_pack_set(W, m, slot, pack); W.flags |= AF_FLAG_LB_EMPTY; }
                     else {
                         uint32_t pick = w32_ld(m, lb);
                         if (C.lb_algo == AF_LB_ROUND_ROBIN) {      // lb_algorithms.py:22-36
@@ -1105,7 +1145,7 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                 act = A_SEND;
                 break;
             }
-            if (act != A_SEND) rq_pack_set(m, slot, pack);   // the request yields here: its record goes back (SEND stores its own)
+            if (act != A_SEND) rq_pack_set(W, m, slot, pack);   // the request yields here: its record goes back (SEND stores its own)
         }
         AFL_SYNC();
 
@@ -1191,7 +1231,7 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                     c32_st(m, C.c_drop + (int32_t)edge, c32_ld(m, C.c_drop + (int32_t)edge) + 1);
                     rq_release(W, m, slot);
                 } else {
-                    rq_pack_set(m, slot, pack);              // (the one store of the record on the request's way out of a node)
+                    rq_pack_set(W, m, slot, pack);              // (the one store of the record on the request's way out of a node)
                     conn_add(W, m, edge, 1);
                     double effective = transit;
                     if (C.n_spike > 0) effective = transit + f64_ld(m, C.o64_spike + (int32_t)edge);   // spike read at SEND time (edge.py:94-106)

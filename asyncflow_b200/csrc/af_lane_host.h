@@ -94,17 +94,37 @@ inline std::vector<int32_t> column_aliases(const double* values, uint64_t n_rows
     return alias;
 }
 
-// How many pending events a replica of this launch typically holds: Little's law on the scenario (and the sweep's
-// largest values) -- requests in flight = arrival rate x time in system, one pending event each, plus the generator's
-// and the injection timelines' own.  Only used to split a lane's shared memory (a wrong guess costs speed, not results).
-inline int32_t pending_events_estimate(const AfScenario& s, const AfSweep* sw) {
-    double users = s.users_mean, rate = s.rate_per_user, edge = 0.0, steps = 0.0;
+// How many pending events a replica typically holds: Little's law -- requests in flight = arrival rate x time in
+// system (`edge`: the longest mean edge latency, `steps`: the longest endpoint), one pending event each, plus the
+// generator's and the injection timelines' own.  Only used to split a lane's shared memory (a wrong guess costs speed,
+// not results).
+inline int32_t littles_law_events(const AfScenario& s, double users, double rate, double edge, double steps) {
+    const int hops = s.n_lb_edges > 0 ? 4 : 3;           // generator -> client -> [LB ->] server -> client
+    const double in_flight = users * rate * (hops * edge + steps);
+    const double need = in_flight + 6.0;
+    return need > 100000.0 ? 100000 : (int32_t)need;
+}
+inline double longest_edge(const AfScenario& s) {
+    double edge = 0.0;
     for (int i = 0; i < s.n_edges; ++i) if (s.edges[i].mean > edge && s.edges[i].dist != AF_DIST_LOG_NORMAL) edge = s.edges[i].mean;
+    return edge;
+}
+// the longest endpoint: step durations from `dur` (one per step)
+inline double longest_endpoint(const AfScenario& s, const double* dur) {
+    double steps = 0.0;
     for (int e = 0; e < s.n_endpoints; ++e) {
         double d = 0.0;
-        for (int k = 0; k < s.endpoints[e].n_steps; ++k) d += s.steps[s.endpoints[e].step_begin + k].duration;
+        for (int k = 0; k < s.endpoints[e].n_steps; ++k) d += dur[s.endpoints[e].step_begin + k];
         if (d > steps) steps = d;
     }
+    return steps;
+}
+// ... of the scenario, with the sweep's largest users, rates and edge means (the launch's heaviest replica at most)
+inline int32_t pending_events_estimate(const AfScenario& s, const AfSweep* sw) {
+    double users = s.users_mean, rate = s.rate_per_user, edge = longest_edge(s);
+    std::vector<double> dur((size_t)s.n_steps);
+    for (int k = 0; k < s.n_steps; ++k) dur[(size_t)k] = s.steps[k].duration;
+    const double steps = longest_endpoint(s, dur.data());
     if (sw)
         for (int c = 0; c < sw->n_columns; ++c) {
             const int f = sw->columns[c].field;
@@ -113,10 +133,41 @@ inline int32_t pending_events_estimate(const AfScenario& s, const AfSweep* sw) {
             for (uint64_t r = 0; r < sw->n_rows; ++r) { const double v = sw->values[r * (uint64_t)sw->n_columns + (uint64_t)c]; if (v > mx) mx = v; }
             if (f == AF_FIELD_USERS_MEAN) users = mx; else if (f == AF_FIELD_RATE_PER_USER) rate = mx; else if (mx > edge) edge = mx;
         }
-    const int hops = s.n_lb_edges > 0 ? 4 : 3;           // generator -> client -> [LB ->] server -> client
-    const double in_flight = users * rate * (hops * edge + steps);
-    const double need = in_flight + 6.0;
-    return need > 100000.0 ? 100000 : (int32_t)need;
+    return littles_law_events(s, users, rate, edge, steps);
+}
+// ... of every row of the sweep, on the row's own values (swept users, rate, edge means, step durations): out[r].
+// The lane kernel splits each replica's pool by its row's estimate.  Returns the largest.
+inline int32_t row_events_estimates(const AfScenario& s, const AfSweep& sw, std::vector<int32_t>& out) {
+    out.assign((size_t)sw.n_rows, 0);
+    std::vector<double> mean((size_t)s.n_edges), dur((size_t)s.n_steps);
+    bool per_row_steps = false;
+    for (int c = 0; c < sw.n_columns; ++c) per_row_steps = per_row_steps || sw.columns[c].field == AF_FIELD_STEP_DURATION;
+    for (int k = 0; k < s.n_steps; ++k) dur[(size_t)k] = s.steps[k].duration;
+    double steps = longest_endpoint(s, dur.data());
+    int32_t mx = 0;
+    for (uint64_t r = 0; r < sw.n_rows; ++r) {
+        const double* row = sw.values + r * (uint64_t)sw.n_columns;
+        double users = s.users_mean, rate = s.rate_per_user;
+        for (int i = 0; i < s.n_edges; ++i) mean[(size_t)i] = s.edges[i].mean;
+        if (per_row_steps) for (int k = 0; k < s.n_steps; ++k) dur[(size_t)k] = s.steps[k].duration;
+        for (int c = 0; c < sw.n_columns; ++c) {            // (two columns over one field: the later one wins, as in the kernels)
+            const int i = sw.columns[c].index;
+            switch (sw.columns[c].field) {
+            case AF_FIELD_USERS_MEAN: users = row[c]; break;
+            case AF_FIELD_RATE_PER_USER: rate = row[c]; break;
+            case AF_FIELD_EDGE_MEAN: mean[(size_t)i] = row[c]; break;
+            case AF_FIELD_STEP_DURATION: dur[(size_t)i] = row[c]; break;
+            default: break;
+            }
+        }
+        double edge = 0.0;
+        for (int i = 0; i < s.n_edges; ++i) if (mean[(size_t)i] > edge && s.edges[i].dist != AF_DIST_LOG_NORMAL) edge = mean[(size_t)i];
+        if (per_row_steps) steps = longest_endpoint(s, dur.data());
+        const int32_t need = littles_law_events(s, users, rate, edge, steps);
+        out[(size_t)r] = need;
+        if (need > mx) mx = need;
+    }
+    return mx;
 }
 
 constexpr int32_t LANE_EVENT_CAPACITY = 512;      // defaults of the lane engine's global tiers (AfOptions fields <= 0)
@@ -131,12 +182,19 @@ inline int32_t fixed_lane_bytes(const AfScenario& s, const Tables& t) {
     const int32_t fix32 = s.n_edges + afl::SV_WORDS * s.n_servers + s.n_lb_edges + (n_series + 31) / 32;
     return 8 * fix64 + 4 * fix32;
 }
-constexpr int32_t MIN_DYNAMIC_BYTES = 16 * 4 + 36 * 2;      // make_cfg: rq_s = (rest - 64) / 36 >= 2
+constexpr int32_t MIN_DYNAMIC_BYTES = 16 * 4 + 36 * 2;      // (a pool of 8 elements: 4 heap entries, 2 records and more)
 // smallest per-lane budget make_cfg() accepts for this scenario
 inline int32_t min_lane_bytes(const AfScenario& s, const Tables& t) { return fixed_lane_bytes(s, t) + MIN_DYNAMIC_BYTES; }
 
-// `ev_need`: pending_events_estimate() of the launch (0: split evenly -- the twin's default); `rq_min`: the record slots
-// that stay in shared memory when the events take the rest.
+// The split of the lane's pool a replica with an estimated `need` pending events gets: {ev_s, rq_s}
+inline void pool_split(const afl::Cfg& C, int32_t need, int32_t& ev_s, int32_t& rq_s) {
+    ev_s = afl::pool_events(C.pool, C.ev_lo, C.rq_floor, C.ev_total, C.rq_total, need);
+    rq_s = C.pool - ev_s;
+}
+
+// `ev_need`: pending-events estimate of the replicas the launch has no per-replica estimate for (Cfg.row_need; 0: the
+// even split -- the twin's default); `rq_min`: the record slots that stay in shared memory when the events take more
+// than the even split.
 // The launch configuration for a budget of `lane_bytes` of shared memory per lane (= per replica in
 // flight).  Returns false when even the smallest tiers do not fit: the topology is too wide for this
 // engine at this occupancy (the caller lowers the occupancy or takes the warp-per-replica engine).
@@ -161,58 +219,46 @@ inline bool make_cfg(const AfScenario& s, const AfOptions& o, const Tables& t, i
     C.n_dirty = (C.n_series + 31) / 32;
     const int32_t fix32 = C.n_edges + afl::SV_WORDS * C.n_servers + C.n_lb_edges + C.n_dirty;
     int32_t nq_s = 0;                                // zero-delay items: ties only -- the ring starts in the global tier
-    int32_t rest = lane_bytes - 8 * fix64 - 4 * fix32;
-    // split the rest between pending events (16 B) and request records (20 B): at nominal load a request in
-    // flight owns one pending event, plus the arrival and the two timelines
-    int32_t rq_s = (rest - 16 * 4) / 36;
-    if (ev_need > 0) {
-        // Heap entries are touched ~20 times per event, a request record twice: when a replica typically holds more
-        // pending events than the even split keeps in shared memory, the events get the bytes, down to `rq_min` (2)
-        // record slots, and never BELOW the even split (scenarios whose events already fit lose record slots for
-        // nothing).
-        const int32_t ev_even = (rest - 20 * rq_s) / 16;
-        if (rq_min < 2) rq_min = 2;
-        int32_t ev_try = ev_need, ev_max = (rest - 20 * rq_min) / 16;
-        if (ev_try > ev_max) ev_try = ev_max;
-        if (ev_try > ev_total) ev_try = ev_total;
-        if (ev_try > ev_even) {
-            const int32_t rq_try = (rest - 16 * ev_try) / 20;
-            if (rq_try >= 2) rq_s = rq_try;
-        }
-    }
-    if (rq_s > rq_total) rq_s = rq_total;
-    int32_t ev_s = rq_s < 0 ? 0 : (rest - 20 * rq_s) / 16;
-    if (ev_s > ev_total) { ev_s = ev_total; rq_s = (rest - 16 * ev_s) / 20; if (rq_s > rq_total) rq_s = rq_total; }
-    if (rq_s < (rq_total < 2 ? rq_total : 2) || ev_s < (ev_total < 4 ? ev_total : 4)) return false;
-    if (ev_s == ev_total && rq_s == rq_total) {      // everything fits: what is left over takes the front of the now-queue
-        nq_s = (rest - 16 * ev_s - 20 * rq_s) / 8;
+    const int32_t rest = lane_bytes - 8 * fix64 - 4 * fix32;
+    // the rest is the pool: 16-byte elements shared by the heap and the request records, split per replica
+    // (afl::pool_events); it never holds more than both tables can use
+    const int32_t rq_cap = rq_total < afl::RQ_BITS ? rq_total : afl::RQ_BITS;
+    int32_t pool = rest < 0 ? 0 : rest / 16;
+    if (pool > ev_total + rq_cap) {                  // everything fits: what is left over takes the front of the now-queue
+        pool = ev_total + rq_cap;
+        nq_s = (rest - 16 * pool) / 8;
         if (nq_s > afl::NQ_TOTAL) nq_s = afl::NQ_TOTAL;
-        if (nq_s < 0) nq_s = 0;
     }
-    C.ev_s = ev_s; C.ev_total = ev_total; C.rq_s = rq_s; C.rq_total = rq_total; C.nq_s = nq_s;
-    C.o128_ev = 0; C.o128_rq = ev_s; C.n128 = ev_s + rq_s;
+    if (pool < (ev_total < 4 ? ev_total : 4) + (rq_total < 2 ? rq_total : 2)) return false;
+    // The even split -- at nominal load a request in flight owns one pending event, plus the arrival and the two
+    // timelines -- is the fewest heap entries a replica gets: a replica whose events fit does not need the record slots
+    // beyond it.  Above it the heap takes what the replica's estimate asks for, down to `rq_min` (>= 2) record slots.
+    C.pool = pool; C.ev_lo = pool - (pool - 4) / 2; C.rq_floor = rq_min < 2 ? 2 : rq_min;
+    C.row_need = nullptr; C.need_first = 0; C.need_rows = 0;
+    C.ev_total = ev_total; C.rq_total = rq_total; C.nq_s = nq_s;
+    pool_split(C, ev_need, C.ev_s, C.rq_s);
+    C.n128 = pool;
     int32_t e = 0;
     C.o64_nq = e; e += nq_s;
     C.o64_spike = e; e += C.n_spike > 0 ? C.n_edges : 0;
     C.o64_row = e; e += C.n_row;
     C.n64 = e;
     int32_t w = 0;
-    C.o32_next = w; w += rq_s;
     C.o32_conn = w; w += C.n_edges;
     C.o32_srv = w; w += afl::SV_WORDS * C.n_servers;
     C.o32_lb = w; w += C.n_lb_edges;
     C.o32_dirty = w; w += C.n_dirty;
     C.n32 = w;
     C.warp_bytes = (C.n128 * 16 + C.n64 * 8 + C.n32 * 4) * lanes;
-    // global tier: 128-bit region (events, request records), 64-bit region (now-queue), 32-bit region (links, cold words)
-    C.gi_ev = 0 - ev_s;
-    C.gi_rq = (ev_total - ev_s) - rq_s;
-    C.gn128 = (ev_total - ev_s) + (rq_total - rq_s);
+    // global tier: 128-bit region (events, request records), 64-bit region (now-queue), 32-bit region (links, cold words).
+    // A replica keeps ev_s + rq_s = pool entries in shared memory whatever its split: heap entries [ev_s, ev_total) at
+    // elements [0, ev_total - ev_s), record slots [rq_s, rq_total) right after them
+    C.gi_rq = ev_total - pool;
+    C.gn128 = ev_total + rq_total - pool;
     C.gi_nq = 0 - nq_s;
     C.gi_acc = afl::NQ_TOTAL - nq_s;
     C.gn64 = C.gi_acc + C.n_series;
-    C.gi_next = 0 - rq_s;
-    int32_t hcount = rq_total - rq_s;
+    int32_t hcount = rq_total;                       // the `next` link of every record slot
     C.g32_cold = hcount;
     C.c_srvq = 0; C.c_inbox = C.c_srvq + afl::SQ_WORDS * C.n_servers; C.c_drop = C.c_inbox + afl::IB_WORDS * (C.n_servers + 2);
     hcount += C.c_drop + C.n_edges;

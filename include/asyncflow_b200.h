@@ -38,7 +38,7 @@
 extern "C" {
 #endif
 
-#define AF_ABI_VERSION 1
+#define AF_ABI_VERSION 2
 
 typedef enum AfStatus {
     AF_OK = 0,
@@ -231,9 +231,13 @@ typedef struct AfRunPasses {
     int32_t lane_pass, warp_pass;        /* which kernels ran                                            */
     int32_t lane_warps_per_sm;           /* occupancy the lane pass chose                                */
     int32_t lane_bytes;                  /* shared memory per replica in flight                          */
-    int32_t lane_events_smem, lane_requests_smem;   /* pool entries kept in shared memory               */
+    int32_t lane_events_smem, lane_requests_smem;   /* split of the lane's shared-memory pool between heap
+                                                       entries and request records, for the launch's
+                                                       heaviest replica (each replica is split by its own
+                                                       estimated load)                                  */
     uint64_t lane_replicas;              /* replicas the thread-per-replica pass ran                     */
     uint64_t warp_replicas;              /* replicas the warp-per-replica pass ran (AUTO: the flagged)   */
+    int32_t lane_pool_elems;             /* 16-byte elements of a lane's pool (heap entries + records)   */
 } AfRunPasses;
 int af_last_run_passes(af_engine* e, AfRunPasses* out);
 

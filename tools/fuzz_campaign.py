@@ -24,13 +24,14 @@ LAYOUTS = False
 
 def layout_for(seed: int) -> dict:
     """A per-seed shared-memory layout for the lane engine: the budget of one lane (the CUDA engine runs 600-1800 B per
-    lane, depending on the occupancy it picks) and the pending-events estimate that splits it (af_run: Little's law)."""
+    lane, depending on the occupancy it picks), and a random split of the lane's pool for every replica (2 .. pool - 1
+    record slots: af_run splits each replica by its own estimated load)."""
     if not LAYOUTS or ENGINE != "lane":
         return {}
     import random
     r = random.Random(seed * 7919 + 13)
     return {"lane_bytes": r.choice([1, 300, 420, 520, 604, 648, 660, 900, 1200, 1816]),     # 1: the smallest the scenario fits in
-            "ev_need": r.choice([0, 0, 4, 12, 26, 60, 200, 100000])}
+            "split": "random", "split_seed": seed}
 
 
 def one(seed: int):
@@ -44,8 +45,14 @@ def one(seed: int):
         payload = fuzz.big_scenario(seed) if BIG else fuzz.scenario(seed)
         flat = flatten(payload)
         o = des_port.simulate(payload, seed=SEED, replica=seed)
-        r = twin.run(flat, seed=SEED, replica_begin=seed, n=1, trace=1, clock_cap=200000, request_capacity=400000,
-                     event_capacity=8192, engine=ENGINE, **layout_for(seed))
+        kw = dict(seed=SEED, replica_begin=seed, n=1, trace=1, clock_cap=200000, request_capacity=400000,
+                  event_capacity=8192)
+        layout = layout_for(seed)
+        if layout:          # tests/split_twin.py: the lane state machine with a split of its pool per replica
+            import split_twin
+            r = split_twin.run(flat, **kw, **layout)
+        else:
+            r = twin.run(flat, engine=ENGINE, **kw)
         st = r["stats"][0]
         n, nt = int(st["completed"]), int(st["n_ticks"])
         assert st["flags"] == 0, f"flags {int(st['flags'])}"
@@ -64,12 +71,15 @@ def main() -> None:
     ap.add_argument("--engine", default="lane", choices=["lane", "warp"], help="which state machine of tests/twin.py")
     ap.add_argument("--big", action="store_true", help="C5-shaped topologies (fuzz.big_scenario)")
     ap.add_argument("--layouts", action="store_true",
-                    help="lane engine: a random per-lane shared-memory budget and split per seed (both tiers of every table)")
+                    help="lane engine: a random per-lane shared-memory budget per seed, a random split of the pool per replica (both tiers of every table)")
     a = ap.parse_args()
     global ENGINE, BIG, LAYOUTS
     ENGINE, BIG, LAYOUTS = a.engine, a.big, a.layouts
     import twin
     twin.build()
+    if LAYOUTS and ENGINE == "lane":
+        import split_twin
+        split_twin.lib()                # built once, before the workers fork
     bad = []
     total = 0
     with mp.get_context("fork").Pool(a.jobs) as pool:
