@@ -230,6 +230,7 @@ struct Globals {
     uint32_t* hist; uint32_t* thr; uint64_t* samp_sum; uint32_t* samp_max;
     double* trace_clocks; uint32_t* trace_series; uint32_t* trace_counts;
     unsigned long long* work_counter;
+    const uint32_t* order;           // first pass: the k-th replica a warp pulls is local index order[k] (af_run)
     // second pass (af_engine.cu): the replicas the thread-per-replica pass flagged; NULL = every replica of the launch
     const uint32_t* redo_list; const uint32_t* redo_count;
     uint64_t seed, replica_begin, n_replicas;

@@ -4,7 +4,8 @@
 //   af_lane_kernel        one replica per THREAD (af_lane.cuh).  One persistent CTA of up to 12 warps per SM; a
 //                         lane's mutable state is element-interleaved in shared memory (conflict-free however far
 //                         the 32 replicas of a warp drift apart), deep tiers and write-only aggregates in global
-//                         memory; lanes pull replica indices from a global counter.  af_run uses it when the launch
+//                         memory; lanes pull replica indices from a global counter through the pull order
+//                         (af_order_key_kernel + radix sorts: heaviest first).  af_run uses it when the launch
 //                         has replicas for most lanes (AF_MODE_AUTO: n >= 3 x SMs x 32) and the topology leaves it
 //                         at least 4 warps per SM.
 //   af_flagged_kernel     compacts the replicas that overflowed the lane kernel's tiers (sized for nominal load)
@@ -28,8 +29,16 @@
 #include <string>
 #include <vector>
 
+#include <cub/device/device_radix_sort.cuh>
+
 #include "af_host_common.h"
 #include "af_lane_host.h"
+
+// Per-event cost of a replica in units of one event it keeps pending: an event costs AF_ORDER_EVENT_COST + need.
+// Least-squares fit of lane time per event against the row's estimate on the bench workload (H100, DESIGN.md §6).
+#ifndef AF_ORDER_EVENT_COST
+#define AF_ORDER_EVENT_COST 44.0
+#endif
 
 // thread-per-replica pass: most warps per SM when the caller does not say (AfOptions.warps_per_block); af_run lowers it
 // to whole waves and to what the topology's fixed tables leave room for (12: see af_lane_kernel)
@@ -67,6 +76,7 @@ __global__ void AF_LAUNCH_BOUNDS af_sim_kernel() {
             if (r >= (unsigned long long)*afc::c_G.redo_count) break;
             r = afc::c_G.redo_list[r];
         } else if (r >= afc::c_G.n_replicas) break;
+        else r = afc::c_G.order[r];
         afc::run_replica(W, (uint64_t)r);
         __syncwarp();
     }
@@ -93,7 +103,7 @@ __global__ void __launch_bounds__(AF_LANE_MAX_THREADS, 1) af_lane_kernel() {
     afl::run_lane(m,
         [&]() -> uint64_t {
             const unsigned long long k = atomicAdd(C.work_counter, 1ull);
-            return k < C.n_replicas ? (uint64_t)k : ~0ull;
+            return k < C.n_replicas ? (uint64_t)C.order[k] : ~0ull;
         },
         [](bool alive) -> bool { return __any_sync(0xFFFFFFFFu, alive) != 0; });
 }
@@ -103,6 +113,51 @@ __global__ void af_flagged_kernel(const AfReplicaStats* __restrict__ stats, uint
                                   uint32_t* __restrict__ list, uint32_t* __restrict__ count) {
     const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n && (stats[i].flags & mask)) list[atomicAdd(count, 1u)] = (uint32_t)i;
+}
+
+// ---- pull order ------------------------------------------------------------------------------------------------
+// A lane runs replicas back to back, and the launch ends when its last lane does.  Pulled in id order, the heaviest
+// replicas of a sweep tend to come last and the launch ends on a few busy lanes; the simulation kernels therefore pull
+// local indices through an order: heaviest first by each replica's predicted work (DESIGN.md §3.3).  Which lane runs a
+// replica, and when, changes no result: its random numbers are keyed by its replica id, its outputs by its local index.
+struct OrderArgs {
+    const AfSweepColumn* cols; const double* vals; int32_t n_cols; uint64_t sweep_first, sweep_rows;
+    const int32_t* row_need; int32_t need;     // per-row pending-events estimates (nullptr: `need` for every replica)
+    uint64_t seed, begin, n;
+    int32_t users_dist; double users_mean, users_sigma, rate_per_user, span;   // span: the first window, at most the horizon
+};
+
+// the replica's pending-events estimate: its row's, else the scenario's
+__device__ __forceinline__ int32_t order_need(const OrderArgs& a, uint64_t i) {
+    const uint64_t r = a.begin + i - a.sweep_first;
+    return a.row_need != nullptr && r < a.sweep_rows ? a.row_need[r] : a.need;
+}
+
+// Predicted work of a replica: the requests of its first window -- the users it draws at t = 0 (the same draw its
+// generator makes) x rate x window -- times the per-event cost of its load, which grows with the events it keeps
+// pending (measured: DESIGN.md §3.3).  Non-negative floats: the bits sort as the values.
+__global__ void af_order_key_kernel(const OrderArgs a, uint32_t* __restrict__ key, uint32_t* __restrict__ idx) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= a.n) return;
+    const uint64_t replica = a.begin + i, r = replica - a.sweep_first;
+    double um = a.users_mean, us = a.users_sigma, rate = a.rate_per_user;
+    if (r < a.sweep_rows)
+        for (int32_t c = 0; c < a.n_cols; ++c) afl::gen_field(a.cols[c].field, a.vals[r * (uint64_t)a.n_cols + (uint64_t)c], um, us, rate);
+    const double users = afr::gen_users(a.seed, replica, 0u, a.users_dist, um, us).value;
+    const double cost = users * rate * a.span * (AF_ORDER_EVENT_COST + (double)order_need(a, i));
+    key[i] = cost > 0.0 ? __float_as_uint((float)cost) : 0u;
+    idx[i] = (uint32_t)i;
+}
+
+// The first wave (the heaviest `lanes` replicas) again, grouped by estimate, then by work: the 32 lanes of a warp start
+// replicas with the same split of the pool and similar loads.  key64 = estimate : work.
+__global__ void af_order_group_kernel(const OrderArgs a, const uint32_t* __restrict__ key, const uint32_t* __restrict__ order,
+                                      uint64_t lanes, uint64_t* __restrict__ key64, uint32_t* __restrict__ idx) {
+    const uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= lanes) return;
+    const uint32_t i = order[j];
+    key64[j] = ((uint64_t)(uint32_t)order_need(a, i) << 32) | key[j];
+    idx[j] = i;
 }
 
 // AF-RNG on the device, outside the state machine: what tests/test_gpu_rng.py compares with oracle/afrng_c
@@ -273,6 +328,7 @@ struct af_engine {
     bool last_lane = false, last_warp = false; int last_lane_warps = 0;
     // spill + outputs
     DevBuf d_sp_evt, d_sp_evk, d_sp_rq, d_sp_nx;
+    DevBuf d_okey, d_oidx, d_order, d_okey64, d_sort_tmp;     // pull order (af_order_*_kernel + radix sorts)
     DevBuf d_stats, d_sent, d_dropped, d_hist, d_thr, d_ssum, d_smax, d_tclk, d_tser, d_tcnt, d_counter, d_htot;
     // last run
     uint64_t last_n = 0; bool ran = false;
@@ -350,7 +406,8 @@ void af_engine_destroy(af_engine* e) {
                       &e->d_edges, &e->d_servers, &e->d_eps, &e->d_steps, &e->d_lb, &e->d_spikes, &e->d_outages,
                       &e->d_sweep_cols, &e->d_sweep_vals, &e->d_row_need, &e->d_sp_evt, &e->d_sp_evk, &e->d_sp_rq, &e->d_sp_nx,
                       &e->d_stats, &e->d_sent, &e->d_dropped, &e->d_hist, &e->d_thr, &e->d_ssum, &e->d_smax,
-                      &e->d_tclk, &e->d_tser, &e->d_tcnt, &e->d_counter, &e->d_htot};
+                      &e->d_tclk, &e->d_tser, &e->d_tcnt, &e->d_counter, &e->d_htot,
+                      &e->d_okey, &e->d_oidx, &e->d_order, &e->d_okey64, &e->d_sort_tmp};
     for (DevBuf* b : bufs) b->release();
     cudaEventDestroy(e->ev_begin); cudaEventDestroy(e->ev_sim); cudaEventDestroy(e->ev_end);
     cudaStreamDestroy(e->stream);
@@ -608,6 +665,28 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
         AF_CUDA(e, e->d_tser.ensure(ntr * (uint64_t)L.n_series * (uint64_t)L.trace_tick_cap * 4 + 4), "trace series");
     }
     AF_CUDA(e, e->d_tcnt.ensure((ntr ? ntr : 1) * 8), "trace counts");
+    // pull order: the first pass runs `workers` replicas at once (lanes, or warps without the thread-per-replica pass)
+    const uint64_t workers = lane ? lgrid * (uint64_t)lane_warps * 32ull : warp_slots;
+    const uint64_t wave = workers < n ? workers : n;
+    size_t sort_bytes = 0, sort2_bytes = 0;
+    AF_CUDA(e, cub::DeviceRadixSort::SortPairsDescending(nullptr, sort_bytes, (const uint32_t*)nullptr, (uint32_t*)nullptr,
+                                                         (const uint32_t*)nullptr, (uint32_t*)nullptr, (uint32_t)n, 0, 32, e->stream), "order sort size");
+    AF_CUDA(e, cub::DeviceRadixSort::SortPairsDescending(nullptr, sort2_bytes, (const uint64_t*)nullptr, (uint64_t*)nullptr,
+                                                         (const uint32_t*)nullptr, (uint32_t*)nullptr, (uint32_t)wave, 0, 64, e->stream), "order sort size");
+    AF_CUDA(e, e->d_okey.ensure(n * 8), "pull order keys");
+    AF_CUDA(e, e->d_oidx.ensure(n * 4), "pull order");
+    AF_CUDA(e, e->d_order.ensure(n * 4), "pull order");
+    AF_CUDA(e, e->d_okey64.ensure(wave * 16), "pull order keys");
+    AF_CUDA(e, e->d_sort_tmp.ensure(sort_bytes > sort2_bytes ? sort_bytes : sort2_bytes), "pull order sort");
+    OrderArgs oa;
+    memset(&oa, 0, sizeof oa);
+    oa.cols = (const AfSweepColumn*)e->d_sweep_cols.p; oa.vals = (const double*)e->d_sweep_vals.p; oa.n_cols = e->sweep_cols;
+    oa.sweep_first = e->sweep_first; oa.sweep_rows = e->sweep_cols ? e->sweep_rows : 0;
+    oa.row_need = e->sweep_cols ? (const int32_t*)e->d_row_need.p : nullptr; oa.need = e->ev_need;
+    oa.seed = seed; oa.begin = begin; oa.n = n;
+    oa.users_dist = e->sc.users_dist; oa.users_mean = e->sc.users_mean; oa.users_sigma = e->sc.users_sigma;
+    oa.rate_per_user = e->sc.rate_per_user;
+    oa.span = (double)(e->sc.window_s < e->sc.horizon_s ? e->sc.window_s : e->sc.horizon_s);   // only the first window is predicted
 
     afc::Globals G;
     memset(&G, 0, sizeof G);
@@ -624,6 +703,7 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
     G.samp_sum = (uint64_t*)e->d_ssum.p; G.samp_max = (uint32_t*)e->d_smax.p;
     G.trace_clocks = (double*)e->d_tclk.p; G.trace_series = (uint32_t*)e->d_tser.p; G.trace_counts = (uint32_t*)e->d_tcnt.p;
     G.work_counter = (unsigned long long*)e->d_counter.p;
+    G.order = (const uint32_t*)e->d_order.p;
     G.redo_list = redo ? (const uint32_t*)e->d_redo_list.p : nullptr;
     G.redo_count = redo ? (const uint32_t*)e->d_redo_count.p : nullptr;
     G.seed = seed; G.replica_begin = begin; G.n_replicas = n;
@@ -639,6 +719,7 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
         C.samp_sum = G.samp_sum; C.samp_max = G.samp_max; C.trace_clocks = G.trace_clocks; C.trace_series = G.trace_series;
         C.trace_counts = G.trace_counts;
         C.work_counter = (unsigned long long*)e->d_counter2.p;
+        C.order = G.order;
         C.seed = seed; C.replica_begin = begin; C.n_replicas = n;
     }
 
@@ -655,6 +736,19 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
     AF_CUDA(e, cudaMemsetAsync(e->d_counter.p, 0, 8, e->stream), "memset");
     if (L.collect_hist) AF_CUDA(e, cudaMemsetAsync(e->d_hist.p, 0, n * AF_HIST_BINS * 4, e->stream), "memset hist");
     if (L.collect_thr) AF_CUDA(e, cudaMemsetAsync(e->d_thr.p, 0, n * (uint64_t)L.horizon_s * 4, e->stream), "memset thr");
+    {   // the pull order: (work, local index) heaviest first; then the first wave grouped by estimate
+        uint32_t* key = (uint32_t*)e->d_okey.p; uint32_t* idx = (uint32_t*)e->d_oidx.p; uint32_t* order = (uint32_t*)e->d_order.p;
+        uint64_t* key64 = (uint64_t*)e->d_okey64.p;
+        af_order_key_kernel<<<(unsigned)((n + 255) / 256), 256, 0, e->stream>>>(oa, key, idx);
+        AF_CUDA(e, cudaGetLastError(), "af_order_key_kernel launch");
+        AF_CUDA(e, cub::DeviceRadixSort::SortPairsDescending(e->d_sort_tmp.p, sort_bytes, key, key + n, idx, order, (uint32_t)n, 0, 32,
+                                                             e->stream), "order sort");
+        af_order_group_kernel<<<(unsigned)((wave + 255) / 256), 256, 0, e->stream>>>(oa, key + n, order, wave, key64, idx);
+        AF_CUDA(e, cudaGetLastError(), "af_order_group_kernel launch");
+        AF_CUDA(e, cub::DeviceRadixSort::SortPairsDescending(e->d_sort_tmp.p, sort2_bytes, key64, key64 + wave, idx, order, (uint32_t)wave,
+                                                             0, 64, e->stream), "order sort");
+        e->launches += 4;
+    }
     if (lane) {
         AF_CUDA(e, cudaMemsetAsync(e->d_counter2.p, 0, 8, e->stream), "memset");
         AF_CUDA(e, cudaMemsetAsync(e->d_redo_count.p, 0, 4, e->stream), "memset");

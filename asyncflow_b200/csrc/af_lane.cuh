@@ -165,6 +165,7 @@ struct Cfg {
     uint32_t* hist; uint32_t* thr; uint64_t* samp_sum; uint32_t* samp_max;
     double* trace_clocks; uint32_t* trace_series; uint32_t* trace_counts;
     unsigned long long* work_counter;
+    const uint32_t* order;                          // the k-th replica a lane pulls is local index order[k] (af_run)
     const uint32_t* redo_list; const uint32_t* redo_count;
     uint64_t seed, replica_begin, n_replicas;
 };
@@ -287,6 +288,16 @@ constexpr uint32_t STOP_FLAGS = AF_FLAG_EVENT_OVERFLOW | AF_FLAG_REQUEST_OVERFLO
 
 // ---- swept parameters ----------------------------------------------------------------------------
 AFL_IN double row_val(const Mem& m, int32_t c) { return f64_ld(m, AFL_C.o64_row + c); }
+// the generator's parameters a sweep column over `field` sets to `v` when a replica starts; false: not one of them.
+// (start_replica, and af_engine.cu's prediction of a replica's work, which must see the same users and rate)
+AFL_IN bool gen_field(int32_t field, double v, double& users_mean, double& users_sigma, double& rate_per_user) {
+    switch (field) {
+    case AF_FIELD_USERS_MEAN: users_mean = v; return true;
+    case AF_FIELD_USERS_SIGMA: users_sigma = v; return true;
+    case AF_FIELD_RATE_PER_USER: rate_per_user = v; return true;
+    default: return false;
+    }
+}
 AFL_IN uint32_t ep_total_ram(const Mem& m, uint32_t ep) {
     const EndpointP p = ro(AFL_C.endpoints + ep);
     return p.c_ram >= 0 ? (uint32_t)row_val(m, p.c_ram) : p.total_ram;
@@ -750,11 +761,8 @@ AFL_IN void start_replica(St& W, const Mem& m, uint64_t local_index) {
         const ColP col = C.cols[c];
         const double v = has_row ? row[c] : col.base;
         if (col.slot >= 0) { f64_st(m, C.o64_row + col.slot, v); continue; }
-        if (!has_row) continue;
+        if (!has_row || gen_field(col.field, v, W.users_mean, W.users_sigma, W.rate_per_user)) continue;
         switch (col.field) {
-        case AF_FIELD_USERS_MEAN: W.users_mean = v; break;
-        case AF_FIELD_USERS_SIGMA: W.users_sigma = v; break;
-        case AF_FIELD_RATE_PER_USER: W.rate_per_user = v; break;
         case AF_FIELD_SERVER_CPU_CORES: i32_st(m, sv_word((uint32_t)col.index, SV_CPU_FREE), (int32_t)v); break;
         case AF_FIELD_SERVER_RAM_MB: i32_st(m, sv_word((uint32_t)col.index, SV_RAM_FREE), (int32_t)v); break;
         default: break;

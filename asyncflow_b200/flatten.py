@@ -284,13 +284,14 @@ def balanced_order(cost: Any, deal: int = 1) -> np.ndarray:
     """Launch order for a skewed sweep: ``order[p]`` = the sweep row that runs at position ``p``
     (= gets replica id ``p``).
 
-    The engine hands replicas to warps in id order through one work counter, so a sweep sorted by
-    ASCENDING load starts its most expensive replicas last and the launch ends with a few warps
-    working alone (SURVEY.md 8d C2: one saturated replica costs as much as the mean warp's whole
-    share).  Heaviest-first (LPT) order removes that tail.  ``deal`` > 1 additionally deals the sorted
-    rows round-robin into ``deal`` consecutive blocks, so that the contiguous replica ranges of
-    ``deal`` GPU ranks (``distributed.shard_bounds``) each get the same mix, heaviest first
-    (SURVEY.md 8e).  Stable: equal costs keep their row order, a flat sweep comes back unchanged.
+    Within one launch the engine already hands replicas to its lanes heaviest first, by each
+    replica's own predicted work (DESIGN.md §3.3), whatever their ids.  What it cannot do is move
+    work between GPU ranks, which run contiguous replica ranges (``distributed.shard_bounds``): a
+    sweep sorted by load gives the last rank the heaviest rows.  ``deal`` > 1 deals the rows, sorted
+    heaviest first (LPT), round-robin into ``deal`` consecutive blocks, so that the ranges of
+    ``deal`` ranks each get the same mix (SURVEY.md 8e).  The permutation changes which replica id,
+    and hence which random numbers, each row gets.  Stable: equal costs keep their row order, a
+    flat sweep comes back unchanged.
     """
     c = np.asarray(cost, dtype=np.float64).ravel()
     by_cost = np.argsort(-c, kind="stable")
