@@ -11,7 +11,7 @@ from __future__ import annotations
 import ctypes as C
 from pathlib import Path
 
-AF_ABI_VERSION = 2
+AF_ABI_VERSION = 3
 AF_HIST_BINS = 4096
 AF_HIST_SUB_BITS = 7
 AF_HIST_MIN_EXP = -20
@@ -131,7 +131,7 @@ EXPORTS = [
     "af_last_run_ms", "af_launch_count", "af_fetch_stats", "af_fetch_edge_counts",
     "af_fetch_histograms", "af_fetch_throughput", "af_fetch_sampled", "af_fetch_trace_clocks",
     "af_fetch_trace_series", "af_reduce_histograms", "af_engine_set_mode", "af_last_run_passes",
-    "af_selftest_rng",
+    "af_selftest_rng", "af_bands_upload", "af_fetch_bands",
 ]
 
 _lib = None
@@ -175,6 +175,8 @@ def load() -> C.CDLL:
     lib.af_engine_set_mode.argtypes = [vp, i32]
     lib.af_last_run_passes.argtypes = [vp, C.POINTER(AfRunPasses)]
     lib.af_selftest_rng.argtypes = [vp, u64, u64, i32, i32, C.c_double, C.c_double, C.c_uint32, u64, vp, vp]
+    lib.af_bands_upload.argtypes = [vp, vp, u64, u64, C.c_uint32]
+    lib.af_fetch_bands.argtypes = [vp, vp, vp, vp, u64, C.POINTER(u64)]
     for name in EXPORTS:
         fn = getattr(lib, name)
         if fn.restype is C.c_int and name not in ("af_abi_version",):

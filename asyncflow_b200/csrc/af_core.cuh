@@ -172,6 +172,10 @@ struct State {
     uint32_t completed, flags, traced, pad0;
     uint64_t n_events;
     double lat_sum, lat_sumsq, lat_min, lat_max;
+    // per-tick bands: the replica's group's difference rows (nullptr: bands off), the first tick it contributes, the
+    // words per difference row, the byte offset of the table of each series' last emitted value (u32, behind the tables)
+    uint64_t* band;
+    uint32_t band_from, band_stride, band_prev_off, band_pad;
 };
 
 // Everything the kernel needs to know about sizes; built on the host.
@@ -191,6 +195,16 @@ struct Layout {
     int32_t off_ev_time, off_ev_key, off_rq_rec, off_rq_next, off_edge, off_server,
             off_endpoint, off_step, off_lb, off_spike, off_outage, off_samp_sum, off_samp_max, off_nq, off_inbox;
     int32_t warp_bytes;
+};
+
+// Per-tick bands of a launch (af_sim_kernel's parameter; stride == 0: off).  As afl::Cfg's band_* (af_lane.cuh):
+// group g's difference rows start at rows + g * group_words; from[local] = the tick from which a re-run of a flagged
+// replica contributes (the thread-per-replica pass contributed the ticks before it); prev_off = byte offset of the
+// table of each series' last emitted value in the warp's workspace (4 * n_series bytes behind Layout.warp_bytes).
+struct BandArgs {
+    uint64_t* rows; const uint32_t* group; const uint32_t* from;
+    uint64_t first, n, group_words;
+    uint32_t groups, stride; int32_t prev_off, pad;
 };
 
 constexpr int32_t NQ_CAP = 128;   // now-queue capacity (power of two)
@@ -272,6 +286,7 @@ AF_TBL(tbl_samp_sum, uint64_t, off_samp_sum)
 AF_TBL(tbl_samp_max, uint32_t, off_samp_max)
 AF_TBL(tbl_nq, uint64_t, off_nq)
 AF_TBL(tbl_inbox, InboxS, off_inbox)
+AF_IN uint32_t* tbl_band_prev(State& W) { return reinterpret_cast<uint32_t*>(reinterpret_cast<unsigned char*>(&W) + W.band_prev_off); }
 
 // ---- warp primitives (a warp of ONE lane on the host) ------------------------
 #if AF_DEVICE_CODE
@@ -283,6 +298,7 @@ __device__ __forceinline__ uint32_t w_ballot(bool p) { return __ballot_sync(AF_F
 __device__ __forceinline__ uint32_t w_shfl(uint32_t v, int src) { return __shfl_sync(AF_FULL, v, src); }
 __device__ __forceinline__ void w_sync() { __syncwarp(); }
 __device__ __forceinline__ void red_add_u32(uint32_t* p, uint32_t v) { atomicAdd(p, v); }
+__device__ __forceinline__ void red_add_u64(uint64_t* p, uint64_t v) { atomicAdd(reinterpret_cast<unsigned long long*>(p), (unsigned long long)v); }
 #else
 constexpr int WARP = 1;
 static inline int lane_id() { return 0; }
@@ -291,6 +307,7 @@ static inline uint32_t w_ballot(bool p) { return p ? 1u : 0u; }
 static inline uint32_t w_shfl(uint32_t v, int) { return v; }
 static inline void w_sync() {}
 static inline void red_add_u32(uint32_t* p, uint32_t v) { *p += v; }
+static inline void red_add_u64(uint64_t* p, uint64_t v) { *p += v; }
 #endif
 
 // ---------------------------------------------------------------------------------
@@ -911,6 +928,11 @@ AF_FN void take_samples(State& W, double t, uint32_t ev_seq) {
     uint32_t tseq = W.tick_seq, nt = W.n_ticks, seq = W.seq;
     const double horizon = W.horizon;
     const bool traced = W.traced != 0;
+    // per-tick bands: from tick band_from on, a series whose value differs from the last one emitted adds the difference
+    // (and that of the squares) at this tick's index of the group's difference rows -- the lane engine's contract,
+    // evaluated at the ticks instead of at the changes; the first tick emits the full value and joins the count
+    uint64_t* const band = W.band;
+    const uint64_t stride = W.band_stride, sq = (uint64_t)n_series * stride;
 #pragma unroll 1
     while ((tick < t || (tick == t && tseq < ev_seq)) && tick < horizon) {
 #pragma unroll 1
@@ -929,13 +951,46 @@ AF_FN void take_samples(State& W, double t, uint32_t ev_seq) {
             if (v > tbl_samp_max(W)[j]) tbl_samp_max(W)[j] = v;
             if (traced && (int32_t)nt < AF_L.trace_tick_cap)
                 AF_G.trace_series[(W.local * (uint64_t)n_series + (uint32_t)j) * (uint64_t)AF_L.trace_tick_cap + nt] = v;
+            if (band != nullptr && nt >= W.band_from) {
+                const uint32_t p = tbl_band_prev(W)[j];
+                if (v != p) {
+                    uint64_t* row = band + (uint64_t)(1 + j) * stride + nt;
+                    red_add_u64(row, (uint64_t)v - (uint64_t)p);
+                    red_add_u64(row + sq, (uint64_t)v * v - (uint64_t)p * p);
+                    tbl_band_prev(W)[j] = v;
+                }
+            }
         }
+        if (band != nullptr && nt == W.band_from && lane == 0) red_add_u64(band + nt, 1u);
         nt += 1;
         tseq = seq++;                                 // the collector re-arms its timeout here
         tick = tick + AF_L.sample_period;
     }
     w_sync();
     W.tick_time = tick; W.tick_seq = tseq; W.n_ticks = nt; W.seq = seq;
+}
+
+// a replica that a stop flag ends leaves its group at the tick it stopped at: its last emitted values and its count
+// are taken back there (nothing was emitted when it stopped before band_from), and the frozen ticks to the horizon add
+// nothing (band = nullptr)
+AF_FN void band_stop(State& W) {
+    AF_SHARED(&W);
+    const int lane = lane_id();
+    const uint64_t n = W.n_ticks, stride = W.band_stride, sq = (uint64_t)AF_L.n_series * stride;
+    if (n > W.band_from) {
+#pragma unroll 1
+        for (int32_t j = lane; j < AF_L.n_series; j += WARP) {
+            const uint64_t p = tbl_band_prev(W)[j];
+            if (p == 0) continue;
+            uint64_t* row = W.band + (uint64_t)(1 + j) * stride + n;
+            red_add_u64(row, 0 - p);
+            red_add_u64(row + sq, 0 - p * p);
+        }
+        if (lane == 0) red_add_u64(W.band + n, ~0ull);
+    }
+    w_sync();
+    W.band = nullptr;
+    w_sync();
 }
 
 // ---------------------------------------------------------------------------------
@@ -1001,6 +1056,7 @@ AF_FN void load_params(State& W) {
     }
 #pragma unroll 1
     for (int32_t i = lane; i < AF_L.n_series; i += WARP) { tbl_samp_sum(W)[i] = 0; tbl_samp_max(W)[i] = 0; }
+    if (W.band != nullptr) for (int32_t i = lane; i < AF_L.n_series; i += WARP) tbl_band_prev(W)[i] = 0;
 #pragma unroll 1
     for (int32_t i = lane; i < AF_L.n_servers + 2; i += WARP) { InboxS b; b.head = b.tail = NIL; b.pending = 1; b.pad = 0; tbl_inbox(W)[i] = b; }
     w_sync();
@@ -1068,7 +1124,7 @@ AF_FN void write_back(State& W) {
 // ---------------------------------------------------------------------------------
 // the replica
 // ---------------------------------------------------------------------------------
-AF_IN void run_replica(State& W, uint64_t local_index) {
+AF_IN void run_replica(State& W, uint64_t local_index, const BandArgs& band) {
     W.local = local_index;
     W.replica = AF_G.replica_begin + local_index;
     W.now = 0.0; W.horizon = (double)AF_L.horizon_s; W.seq = 0;
@@ -1081,6 +1137,13 @@ AF_IN void run_replica(State& W, uint64_t local_index) {
     W.n_ticks = 0; W.completed = 0; W.flags = 0; W.n_events = 0;
     W.lat_sum = 0.0; W.lat_sumsq = 0.0; W.lat_min = afr::u2d(INF_BITS); W.lat_max = 0.0;
     W.traced = (int64_t)local_index < (int64_t)AF_L.trace_replicas ? 1u : 0u;
+    W.band = nullptr; W.band_from = 0; W.band_stride = band.stride; W.band_prev_off = (uint32_t)band.prev_off;
+    if (band.stride) {
+        const uint64_t i = W.replica - band.first;
+        const uint32_t g = i < band.n ? band.group[i] : band.groups;
+        W.band = band.rows + (uint64_t)g * band.group_words;
+        W.band_from = AF_G.redo_list ? band.from[local_index] : 0u;      // a re-run continues where the lane pass stopped
+    }
     w_sync();
     load_params(W);
 
@@ -1146,8 +1209,13 @@ AF_IN void run_replica(State& W, uint64_t local_index) {
         if (W.flags & STOP_FLAGS) break;
     }
     W.n_events = n_events;
+    if (W.band != nullptr && (W.flags & STOP_FLAGS)) band_stop(W);   // before the frozen ticks to the horizon
     take_samples(W, W.horizon, 0u);                   // ticks strictly before the horizon
     write_back(W);
+}
+AF_IN void run_replica(State& W, uint64_t local_index) {
+    const BandArgs off = {};
+    run_replica(W, local_index, off);
 }
 
 }  // namespace afc

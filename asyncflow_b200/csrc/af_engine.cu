@@ -14,6 +14,7 @@
 //                         whole run for small launches and very wide topologies.  One replica per warp,
 //                         persistent CTAs pulling replica indices from a global counter; per-warp workspace in
 //                         shared memory with spill tiers in HBM.
+//   af_band_scan_kernel   per-tick bands (af_bands_upload): the groups' difference rows -> per-tick sums, in place
 //   af_percentile_kernel  HBM-bound pass over the per-replica latency histograms:
 //                         one warp per replica, coalesced 128-byte row reads, warp
 //                         prefix sums, numpy-"linear" p50/p95/p99.
@@ -24,6 +25,7 @@
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
+#include <algorithm>
 #include <mutex>
 #include <new>
 #include <string>
@@ -59,7 +61,7 @@
 // ---------------------------------------------------------------------------------
 // kernels
 // ---------------------------------------------------------------------------------
-__global__ void AF_LAUNCH_BOUNDS af_sim_kernel() {
+__global__ void AF_LAUNCH_BOUNDS af_sim_kernel(const afc::BandArgs band) {
     extern __shared__ __align__(16) unsigned char af_smem[];
     const int warp = (int)(threadIdx.x >> 5);
     const int lane = (int)(threadIdx.x & 31u);
@@ -77,17 +79,19 @@ __global__ void AF_LAUNCH_BOUNDS af_sim_kernel() {
             r = afc::c_G.redo_list[r];
         } else if (r >= afc::c_G.n_replicas) break;
         else r = afc::c_G.order[r];
-        afc::run_replica(W, (uint64_t)r);
+        afc::run_replica(W, (uint64_t)r, band);
         __syncwarp();
     }
 }
 
 // One replica per thread.  Compiled for one CTA of up to 384 threads per SM (the shared-memory budget of a
 // lane decides the CTA size at launch).  More warps shrink each lane's share of shared memory (more of the heap lives
-// in L2), so the register budget is spent at 12 warps: 158 registers on sm_90a, no spills.
+// in L2), so the register budget is spent at 12 warps: 158 registers on sm_90a, no spills.  kBands: the same kernel
+// also accumulating per-tick bands (af_run uses it when groups are uploaded); <false> is the kernel without them.
 #ifndef AF_LANE_MAX_THREADS
 #define AF_LANE_MAX_THREADS 384
 #endif
+template <bool kBands = false>
 __global__ void __launch_bounds__(AF_LANE_MAX_THREADS, 1) af_lane_kernel() {
     const afl::Cfg& C = afl::c_cfg;
     const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
@@ -100,12 +104,34 @@ __global__ void __launch_bounds__(AF_LANE_MAX_THREADS, 1) af_lane_kernel() {
     m.g128 = gs + lane * 16u;
     m.g64 = gs + (size_t)C.gn128 * afl::STRIDE128 + lane * 8u;
     m.g32 = gs + (size_t)C.gn128 * afl::STRIDE128 + (size_t)C.gn64 * afl::STRIDE64 + lane * 4u;
-    afl::run_lane(m,
+    afl::run_lane<kBands>(m,
         [&]() -> uint64_t {
             const unsigned long long k = atomicAdd(C.work_counter, 1ull);
             return k < C.n_replicas ? (uint64_t)C.order[k] : ~0ull;
         },
         [](bool alive) -> bool { return __any_sync(0xFFFFFFFFu, alive) != 0; });
+}
+
+// per-tick bands: the difference rows -> per-tick values, in place.  One warp per row: 32 ticks at a time, a warp prefix
+// sum plus the carry of the ticks before (u64 modular arithmetic: exact, whatever order the lanes added in)
+__global__ void af_band_scan_kernel(uint64_t* __restrict__ rows, uint64_t n_rows, uint64_t stride, uint64_t n_ticks) {
+    const uint64_t row = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const uint32_t lane = threadIdx.x & 31u;
+    if (row >= n_rows) return;
+    uint64_t* r = rows + row * stride;
+    uint64_t carry = 0;
+    for (uint64_t base = 0; base < n_ticks; base += 32) {
+        const uint64_t k = base + lane;
+        uint64_t x = k < n_ticks ? r[k] : 0;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const uint64_t up = __shfl_up_sync(0xFFFFFFFFu, x, d);
+            if ((int)lane >= d) x += up;
+        }
+        x += carry;
+        if (k < n_ticks) r[k] = x;
+        carry = __shfl_sync(0xFFFFFFFFu, x, 31);
+    }
 }
 
 // replicas whose pools overflowed in the thread-per-replica pass -> list for the warp-per-replica pass
@@ -301,6 +327,7 @@ struct af_engine {
     int device = 0;
     int sm_count = 0;
     int max_smem_optin = 0;
+    uint64_t mem_total = 0;     // device memory: the bound on what the band rows may ask for
     cudaStream_t stream = nullptr;
     cudaEvent_t ev_begin = nullptr, ev_sim = nullptr, ev_end = nullptr;
     std::string err;
@@ -336,6 +363,12 @@ struct af_engine {
     afc::Globals G_host{};
     uint64_t launches = 0;
     float ms_total = 0.f, ms_sim = 0.f; bool timing_valid = false;
+    // per-tick bands (af_bands_upload): group of replica band_first + i, n_groups groups (0: bands off); the difference
+    // rows of n_groups + 1 groups (the last: replicas without a group entry), the tick each flagged replica stopped at
+    std::vector<uint32_t> h_band_group; uint64_t band_first = 0; uint32_t band_groups = 0;
+    DevBuf d_band_group, d_band, d_band_from;
+    uint64_t band_swept_ram = 0; int32_t band_swept_server = -1;     // afh::swept_ram_max of the uploaded sweep
+    bool last_bands = false; uint32_t last_band_groups = 0, last_band_ticks = 0; uint64_t last_band_stride = 0;
 
     int fail(int code, const std::string& m) { err = m; return code; }
     int cuda_fail(cudaError_t e, const char* what) {
@@ -379,6 +412,7 @@ int af_engine_create(int device, af_engine** out) {
     af_engine* e = new (std::nothrow) af_engine();
     if (!e) { g_create_error = "host allocation failed"; return AF_ERR_NOMEM; }
     e->device = device; e->sm_count = prop.multiProcessorCount; e->max_smem_optin = (int)prop.sharedMemPerBlockOptin;
+    e->mem_total = (uint64_t)prop.totalGlobalMem;
     if ((ce = cudaSetDevice(device)) != cudaSuccess || (ce = cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking)) != cudaSuccess
         || (ce = cudaEventCreate(&e->ev_begin)) != cudaSuccess || (ce = cudaEventCreate(&e->ev_sim)) != cudaSuccess
         || (ce = cudaEventCreate(&e->ev_end)) != cudaSuccess) {
@@ -407,7 +441,8 @@ void af_engine_destroy(af_engine* e) {
                       &e->d_sweep_cols, &e->d_sweep_vals, &e->d_row_need, &e->d_sp_evt, &e->d_sp_evk, &e->d_sp_rq, &e->d_sp_nx,
                       &e->d_stats, &e->d_sent, &e->d_dropped, &e->d_hist, &e->d_thr, &e->d_ssum, &e->d_smax,
                       &e->d_tclk, &e->d_tser, &e->d_tcnt, &e->d_counter, &e->d_htot,
-                      &e->d_okey, &e->d_oidx, &e->d_order, &e->d_okey64, &e->d_sort_tmp};
+                      &e->d_okey, &e->d_oidx, &e->d_order, &e->d_okey64, &e->d_sort_tmp,
+                      &e->d_band_group, &e->d_band, &e->d_band_from};
     for (DevBuf* b : bufs) b->release();
     cudaEventDestroy(e->ev_begin); cudaEventDestroy(e->ev_sim); cudaEventDestroy(e->ev_end);
     cudaStreamDestroy(e->stream);
@@ -453,6 +488,7 @@ int af_scenario_upload(af_engine* e, const AfScenario* s) {
     e->have_scenario = true;
     e->sweep_cols = 0; e->sweep_rows = 0; e->h_sweep_cols.clear();     // a sweep belongs to the scenario it was built for
     e->ev_need = aflh::pending_events_estimate(e->sc, nullptr); e->row_need_max = 0;
+    e->band_swept_ram = 0; e->band_swept_server = -1;
     e->ran = false;
     return AF_OK;
 }
@@ -462,7 +498,10 @@ int af_sweep_upload(af_engine* e, const AfSweep* sw, uint64_t first_replica) {
     if (!e->have_scenario) return e->fail(AF_ERR_STATE, "af_sweep_upload before af_scenario_upload");
     AF_CUDA(e, cudaSetDevice(e->device), "cudaSetDevice");
     AF_CUDA(e, cudaStreamSynchronize(e->stream), "sync before sweep upload");
-    if (!sw || sw->n_columns == 0 || sw->n_rows == 0) { e->sweep_cols = 0; e->sweep_rows = 0; e->h_sweep_cols.clear(); e->row_need_max = 0; return AF_OK; }
+    if (!sw || sw->n_columns == 0 || sw->n_rows == 0) {
+        e->sweep_cols = 0; e->sweep_rows = 0; e->h_sweep_cols.clear(); e->row_need_max = 0; e->band_swept_ram = 0; e->band_swept_server = -1;
+        return AF_OK;
+    }
     if (!sw->columns || !sw->values) return e->fail(AF_ERR_INVALID, "sweep: null columns/values");
     const AfScenario& s = e->sc;
     for (int c = 0; c < sw->n_columns; ++c) {
@@ -502,6 +541,7 @@ int af_sweep_upload(af_engine* e, const AfSweep* sw, uint64_t first_replica) {
     // each row's own pending-events estimate: the lane kernel splits the replica's shared-memory pool by it.  On the
     // host, here: one pass over the values (as the checks above), and the kernel's start of a replica stays one load
     e->row_need_max = aflh::row_events_estimates(e->sc, *sw, e->h_row_need);
+    e->band_swept_ram = afh::swept_ram_max(sw->columns, sw->n_columns, sw->values, sw->n_rows, e->band_swept_server);
     size_t cb = (size_t)sw->n_columns * sizeof(AfSweepColumn), vb = (size_t)sw->n_columns * sw->n_rows * sizeof(double);
     AF_CUDA(e, e->d_sweep_cols.ensure(cb), "sweep columns");
     AF_CUDA(e, e->d_sweep_vals.ensure(vb), "sweep values");
@@ -512,6 +552,67 @@ int af_sweep_upload(af_engine* e, const AfSweep* sw, uint64_t first_replica) {
             "sweep row estimates H2D");
     AF_CUDA(e, cudaStreamSynchronize(e->stream), "sweep upload");
     e->sweep_cols = sw->n_columns; e->sweep_rows = sw->n_rows; e->sweep_first = first_replica;
+    return AF_OK;
+}
+
+// sumsq of the per-tick bands is a u64 sum of squares: refuse a group size and gauge bound that could wrap it
+static int band_check(af_engine* e, uint64_t group) {
+    std::string what;
+    const uint64_t bound = afh::band_gauge_bound(e->sc, e->opt, e->band_swept_ram, e->band_swept_server, what);
+    if (afh::band_sumsq_fits(group, bound)) return AF_OK;
+    char b[320];
+    snprintf(b, sizeof b, "bands: a group of %llu replicas x (%llu, the bound on a gauge: %s)^2 could wrap the u64 sum of squares; "
+             "use smaller groups", (unsigned long long)group, (unsigned long long)bound, what.c_str());
+    return e->fail(AF_ERR_INVALID, b);
+}
+
+// The band rows of `n_groups` groups for the current scenario: every tick a replica can take needs its word (the kernels
+// index the rows by the tick count, unchecked), and the rows must fit the device.  ticks = the scenario's tick count.
+static int band_shape_check(af_engine* e, uint64_t n_groups, uint32_t& ticks) {
+    std::string why;
+    if (!afh::band_ticks_fit(e->sc, ticks, why)) return e->fail(AF_ERR_INVALID, why);
+    const unsigned __int128 bytes = afh::band_row_bytes(n_groups, 3 * e->sc.n_servers + e->sc.n_edges, ticks);
+    if (bytes > (unsigned __int128)e->mem_total) {
+        char b[240];
+        snprintf(b, sizeof b, "bands: %llu groups x %u ticks need %.3g GB of band rows, more than the device's %.3g GB",
+                 (unsigned long long)n_groups, ticks, (double)bytes / 1e9, (double)e->mem_total / 1e9);
+        return e->fail(AF_ERR_INVALID, b);
+    }
+    return AF_OK;
+}
+
+// the most replicas one group holds among group_of[0 .. n)
+static uint64_t largest_group(const uint32_t* group_of, uint64_t n) {
+    std::vector<uint32_t> g(group_of, group_of + n);
+    std::sort(g.begin(), g.end());
+    uint64_t best = 0;
+    for (uint64_t i = 0, j; i < n; i = j) {
+        for (j = i + 1; j < n && g[j] == g[i]; ++j) {}
+        best = j - i > best ? j - i : best;
+    }
+    return best;
+}
+
+int af_bands_upload(af_engine* e, const uint32_t* group_of, uint64_t n, uint64_t first_replica, uint32_t n_groups) {
+    if (!e) return AF_ERR_INVALID;
+    if (!e->have_scenario) return e->fail(AF_ERR_STATE, "af_bands_upload before af_scenario_upload");
+    AF_CUDA(e, cudaSetDevice(e->device), "cudaSetDevice");
+    AF_CUDA(e, cudaStreamSynchronize(e->stream), "sync before bands upload");
+    if (!group_of) { e->band_groups = 0; e->h_band_group.clear(); return AF_OK; }
+    if (n == 0 || n_groups == 0) return e->fail(AF_ERR_INVALID, "bands: empty group table or n_groups == 0");
+    for (uint64_t i = 0; i < n; ++i)
+        if (group_of[i] >= n_groups) {
+            char b[160]; snprintf(b, sizeof b, "bands: group_of[%llu] = %u is not < n_groups = %u", (unsigned long long)i, group_of[i], n_groups);
+            return e->fail(AF_ERR_INVALID, b);
+        }
+    uint32_t ticks = 0;
+    int rc = band_shape_check(e, n_groups, ticks);
+    if (rc) return rc;
+    if ((rc = band_check(e, largest_group(group_of, n)))) return rc;
+    e->h_band_group.assign(group_of, group_of + n);
+    if ((rc = upload_vec(e, e->d_band_group, e->h_band_group, "band groups"))) return rc;
+    AF_CUDA(e, cudaStreamSynchronize(e->stream), "band groups H2D");
+    e->band_first = first_replica; e->band_groups = n_groups;
     return AF_OK;
 }
 
@@ -599,6 +700,24 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
     memset(&L, 0, sizeof L);
     afh::make_layout(e->sc, e->opt, e->sweep_cols, L);
 
+    // ---- per-tick bands: difference rows of (groups + 1) x (1 + 2 n_series) x (ticks + 1) words -----------------------
+    const bool bands = e->band_groups > 0;
+    uint32_t ticks32 = 0;
+    if (bands) {      // (the scenario, options and sweep may have changed since af_bands_upload)
+        if ((rc = band_shape_check(e, e->band_groups, ticks32))) return rc;
+        const uint64_t lo = begin > e->band_first ? begin : e->band_first;          // this run's replicas with a group
+        const uint64_t hi = end < e->band_first + e->h_band_group.size() ? end : e->band_first + e->h_band_group.size();
+        if ((rc = band_check(e, lo < hi ? largest_group(e->h_band_group.data() + (lo - e->band_first), hi - lo) : 0))) return rc;
+    }
+    const uint64_t band_ticks = ticks32, band_stride = band_ticks + 1;
+    const uint64_t band_group_words = (1 + 2 * (uint64_t)L.n_series) * band_stride;
+    const uint64_t band_words = bands ? ((uint64_t)e->band_groups + 1) * band_group_words : 0;
+    afc::BandArgs band = {};
+    if (bands) {
+        band.prev_off = L.warp_bytes;                       // the warp engine: each series' last emitted value, behind its tables
+        L.warp_bytes += afc::align_up(4 * L.n_series, 16);
+    }
+
     // ---- launch shapes -------------------------------------------------------------------------------------
     // warp-per-replica: persistent CTAs of <= 4 warps (__launch_bounds__(128, AF_MIN_BLOCKS)), as many per SM as fit
     int wpb = 4; size_t smem = 0; uint64_t grid = 0, warp_slots = 0;
@@ -620,9 +739,10 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
     }
     // thread-per-replica: one persistent CTA per SM
     uint64_t lgrid = 0; size_t lsmem = 0;
+    void (*lane_kernel)() = bands ? af_lane_kernel<true> : af_lane_kernel<false>;
     if (lane) {
         lsmem = (size_t)lane_warps * (size_t)C.warp_bytes;
-        AF_CUDA(e, cudaFuncSetAttribute(af_lane_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lsmem), "smem attribute");
+        AF_CUDA(e, cudaFuncSetAttribute(lane_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lsmem), "smem attribute");
         lgrid = (uint64_t)e->sm_count;
         const uint64_t need = (n + (uint64_t)lane_warps * 32 - 1) / ((uint64_t)lane_warps * 32);
         if (lgrid > need) lgrid = need;
@@ -665,6 +785,10 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
         AF_CUDA(e, e->d_tser.ensure(ntr * (uint64_t)L.n_series * (uint64_t)L.trace_tick_cap * 4 + 4), "trace series");
     }
     AF_CUDA(e, e->d_tcnt.ensure((ntr ? ntr : 1) * 8), "trace counts");
+    if (bands) {
+        AF_CUDA(e, e->d_band.ensure(band_words * 8), "band rows");
+        AF_CUDA(e, e->d_band_from.ensure(n * 4), "band stop ticks");
+    }
     // pull order: the first pass runs `workers` replicas at once (lanes, or warps without the thread-per-replica pass)
     const uint64_t workers = lane ? lgrid * (uint64_t)lane_warps * 32ull : warp_slots;
     const uint64_t wave = workers < n ? workers : n;
@@ -707,6 +831,11 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
     G.redo_list = redo ? (const uint32_t*)e->d_redo_list.p : nullptr;
     G.redo_count = redo ? (const uint32_t*)e->d_redo_count.p : nullptr;
     G.seed = seed; G.replica_begin = begin; G.n_replicas = n;
+    if (bands) {
+        band.rows = (uint64_t*)e->d_band.p; band.group = (const uint32_t*)e->d_band_group.p; band.from = (const uint32_t*)e->d_band_from.p;
+        band.first = e->band_first; band.n = e->h_band_group.size(); band.group_words = band_group_words;
+        band.groups = e->band_groups; band.stride = (uint32_t)band_stride;
+    }
     if (lane) {
         C.edges = (const afl::EdgeP*)e->d_l_edges.p; C.servers = (const afl::ServerP*)e->d_l_servers.p;
         C.endpoints = (const afl::EndpointP*)e->d_l_eps.p; C.steps = (const afl::StepP*)e->d_l_steps.p;
@@ -721,6 +850,11 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
         C.work_counter = (unsigned long long*)e->d_counter2.p;
         C.order = G.order;
         C.seed = seed; C.replica_begin = begin; C.n_replicas = n;
+        if (bands) {
+            C.band_rows = band.rows; C.band_group = band.group; C.band_from = (uint32_t*)e->d_band_from.p;
+            C.band_first = band.first; C.band_n = band.n; C.band_group_words = band_group_words;
+            C.band_groups = (int32_t)e->band_groups; C.band_stride = (int32_t)band_stride;
+        }
     }
 
     // ---- enqueue ---------------------------------------------------------------------------------------------------
@@ -736,6 +870,7 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
     AF_CUDA(e, cudaMemsetAsync(e->d_counter.p, 0, 8, e->stream), "memset");
     if (L.collect_hist) AF_CUDA(e, cudaMemsetAsync(e->d_hist.p, 0, n * AF_HIST_BINS * 4, e->stream), "memset hist");
     if (L.collect_thr) AF_CUDA(e, cudaMemsetAsync(e->d_thr.p, 0, n * (uint64_t)L.horizon_s * 4, e->stream), "memset thr");
+    if (bands) AF_CUDA(e, cudaMemsetAsync(e->d_band.p, 0, band_words * 8, e->stream), "memset band rows");
     {   // the pull order: (work, local index) heaviest first; then the first wave grouped by estimate
         uint32_t* key = (uint32_t*)e->d_okey.p; uint32_t* idx = (uint32_t*)e->d_oidx.p; uint32_t* order = (uint32_t*)e->d_order.p;
         uint64_t* key64 = (uint64_t*)e->d_okey64.p;
@@ -753,7 +888,7 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
         AF_CUDA(e, cudaMemsetAsync(e->d_counter2.p, 0, 8, e->stream), "memset");
         AF_CUDA(e, cudaMemsetAsync(e->d_redo_count.p, 0, 4, e->stream), "memset");
         AF_CUDA(e, cudaMemcpyToSymbolAsync(afl::c_cfg, &C, sizeof C, 0, cudaMemcpyHostToDevice, e->stream), "lane config -> constant memory");
-        af_lane_kernel<<<(unsigned)lgrid, lane_warps * 32, lsmem, e->stream>>>();
+        lane_kernel<<<(unsigned)lgrid, lane_warps * 32, lsmem, e->stream>>>();
         AF_CUDA(e, cudaGetLastError(), "af_lane_kernel launch");
         e->launches += 1;
         if (redo) {
@@ -767,11 +902,17 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
         AF_CUDA(e, cudaMemcpyToSymbolAsync(afc::c_L, &L, sizeof L, 0, cudaMemcpyHostToDevice, e->stream), "layout -> constant memory");
         e->G_host = G;   // keep the source alive until the async copy has been issued from pageable memory
         AF_CUDA(e, cudaMemcpyToSymbolAsync(afc::c_G, &e->G_host, sizeof G, 0, cudaMemcpyHostToDevice, e->stream), "globals -> constant memory");
-        af_sim_kernel<<<(unsigned)grid, wpb * 32, smem, e->stream>>>();
+        af_sim_kernel<<<(unsigned)grid, wpb * 32, smem, e->stream>>>(band);
         AF_CUDA(e, cudaGetLastError(), "af_sim_kernel launch");
         e->launches += 1;
     }
     AF_CUDA(e, cudaEventRecord(e->ev_sim, e->stream), "event");
+    if (bands) {      // the fetched groups' difference rows -> per-tick values (the last group collects replicas without one)
+        const uint64_t rows = (uint64_t)e->band_groups * (1 + 2 * (uint64_t)L.n_series);
+        af_band_scan_kernel<<<(unsigned)((rows * 32 + 255) / 256), 256, 0, e->stream>>>((uint64_t*)e->d_band.p, rows, band_stride, band_ticks);
+        AF_CUDA(e, cudaGetLastError(), "af_band_scan_kernel launch");
+        e->launches += 1;
+    }
     if (L.collect_hist) {
         unsigned blocks = (unsigned)((n * 32 + 255) / 256);
         af_percentile_kernel<<<blocks, 256, 0, e->stream>>>((const uint32_t*)e->d_hist.p, (AfReplicaStats*)e->d_stats.p, n);
@@ -781,6 +922,8 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
     AF_CUDA(e, cudaEventRecord(e->ev_end, e->stream), "event");
     e->last_n = n; e->ran = true; e->timing_valid = false;
     e->last_lane = lane; e->last_warp = warp; e->last_lane_warps = lane_warps;
+    e->last_bands = bands; e->last_band_groups = e->band_groups; e->last_band_ticks = (uint32_t)band_ticks;
+    e->last_band_stride = band_stride;
     return AF_OK;
 }
 
@@ -926,6 +1069,33 @@ int af_fetch_trace_clocks(af_engine* e, uint64_t local, double* out, uint64_t ca
     if (n) AF_CUDA(e, cudaMemcpyAsync(out, (double*)e->d_tclk.p + local * (uint64_t)e->L.trace_clock_cap * 2, n * 16,
                                       cudaMemcpyDeviceToHost, e->stream), "trace clocks");
     return af_sync(e);
+}
+
+int af_fetch_bands(af_engine* e, uint32_t* count, uint64_t* sum, uint64_t* sumsq, uint64_t cap_ticks, uint64_t* n_ticks) {
+    if (!e || !n_ticks) return AF_ERR_INVALID;
+    if (!e->ran) return e->fail(AF_ERR_STATE, "fetch before af_run");
+    if (!e->last_bands) return e->fail(AF_ERR_STATE, "the last run collected no bands (af_bands_upload)");
+    AF_CUDA(e, cudaSetDevice(e->device), "cudaSetDevice");
+    const uint64_t T = e->last_band_ticks, G = e->last_band_groups, S = (uint64_t)e->L.n_series, stride = e->last_band_stride;
+    const uint64_t k = T < cap_ticks ? T : cap_ticks;
+    *n_ticks = T;
+    const uint64_t* base = (const uint64_t*)e->d_band.p;
+    const uint64_t group_words = (1 + 2 * S) * stride;
+    std::vector<uint64_t> c64(count && k ? G * k : 0);
+    for (uint64_t g = 0; g < G && k; ++g) {
+        const uint64_t* gb = base + g * group_words;
+        if (count) AF_CUDA(e, cudaMemcpyAsync(c64.data() + g * k, gb, k * 8, cudaMemcpyDeviceToHost, e->stream), "band counts D2H");
+        if (sum) AF_CUDA(e, cudaMemcpy2DAsync(sum + g * S * cap_ticks, cap_ticks * 8, gb + stride, stride * 8, k * 8, S,
+                                              cudaMemcpyDeviceToHost, e->stream), "band sums D2H");
+        if (sumsq) AF_CUDA(e, cudaMemcpy2DAsync(sumsq + g * S * cap_ticks, cap_ticks * 8, gb + (1 + S) * stride, stride * 8, k * 8, S,
+                                                cudaMemcpyDeviceToHost, e->stream), "band sums of squares D2H");
+    }
+    int rc = af_sync(e);
+    if (rc) return rc;
+    if (count)
+        for (uint64_t g = 0; g < G; ++g)
+            for (uint64_t t = 0; t < k; ++t) count[g * cap_ticks + t] = (uint32_t)c64[g * k + t];
+    return AF_OK;
 }
 
 int af_fetch_trace_series(af_engine* e, uint64_t local, uint32_t* out, uint64_t cap_ticks, uint64_t* n_ticks) {

@@ -80,6 +80,63 @@ inline int32_t trace_tick_capacity(const AfScenario& s) {
     return (int32_t)n + 2;
 }
 
+// Ticks the collector takes before the horizon: n_ticks of every replica that reaches it (the kernels' own repeated
+// addition of the sample period; sample_period is not sweepable, so it is the same for every replica of a scenario).
+// Counted up to BAND_TICK_LIMIT: a result of BAND_TICK_LIMIT means "at least that many" (band_ticks_fit refuses it).
+constexpr uint32_t BAND_TICK_LIMIT = 50000000u;
+inline uint32_t band_ticks(const AfScenario& s) {
+    const double horizon = (double)s.horizon_s;
+    if (horizon / s.sample_period > (double)BAND_TICK_LIMIT + 2.0) return BAND_TICK_LIMIT;
+    uint32_t n = 0;
+    for (double tick = 0.0 + s.sample_period; tick < horizon && n < BAND_TICK_LIMIT; tick = tick + s.sample_period) ++n;
+    return n;
+}
+// The band rows hold one word per tick and the kernels index them by the replica's tick count without a bounds check:
+// every tick a replica can take must have its word, so a scenario that reaches the limit is refused.
+inline bool band_ticks_fit(const AfScenario& s, uint32_t& ticks, std::string& why) {
+    ticks = band_ticks(s);
+    if (ticks < BAND_TICK_LIMIT) return true;
+    why = "bands: horizon " + std::to_string(s.horizon_s) + " s at a sample period of " + std::to_string(s.sample_period) +
+          " s takes " + std::to_string(BAND_TICK_LIMIT) + " ticks or more; per-tick bands hold fewer";
+    return false;
+}
+// bytes of the difference rows of n_groups groups plus the one of the replicas without a group
+inline unsigned __int128 band_row_bytes(uint64_t n_groups, int32_t n_series, uint32_t ticks) {
+    return ((unsigned __int128)n_groups + 1) * (unsigned __int128)(1 + 2 * (uint64_t)n_series) * ((unsigned __int128)ticks + 1) * 8u;
+}
+
+// The largest ram_mb a sweep sets (0: none), and the server it belongs to.
+inline uint64_t swept_ram_max(const AfSweepColumn* cols, int32_t n_cols, const double* vals, uint64_t n_rows, int32_t& server) {
+    uint64_t b = 0;
+    server = -1;
+    for (int32_t c = 0; c < n_cols; ++c) {
+        if (cols[c].field != AF_FIELD_SERVER_RAM_MB) continue;
+        for (uint64_t r = 0; r < n_rows; ++r) {
+            const double v = vals[r * (uint64_t)n_cols + (uint64_t)c];
+            if (v > (double)b) { b = (uint64_t)v; server = cols[c].index; }
+        }
+    }
+    return b;
+}
+
+// The largest value any sampled gauge of a replica can take: a queue length or an edge's connection count is at most
+// the requests in flight (the request capacity of either engine), RAM in use at most the largest ram_mb, swept values
+// (`swept_ram` of server `swept_server`) included.  `what` names the bound that decides.
+inline uint64_t band_gauge_bound(const AfScenario& s, const AfOptions& o, uint64_t swept_ram, int32_t swept_server, std::string& what) {
+    int32_t rq = o.request_capacity > 0 ? o.request_capacity : DEFAULT_REQUEST_CAPACITY;
+    if (rq > (int32_t)afc::SLOT_MASK) rq = (int32_t)afc::SLOT_MASK;
+    uint64_t b = (uint64_t)rq;
+    what = "request capacity " + std::to_string(rq);
+    for (int i = 0; i < s.n_servers; ++i)
+        if ((uint64_t)s.servers[i].ram_mb > b) { b = (uint64_t)s.servers[i].ram_mb; what = "ram_mb " + std::to_string(b) + " of server " + std::to_string(i); }
+    if (swept_ram > b) { b = swept_ram; what = "swept ram_mb " + std::to_string(b) + " of server " + std::to_string(swept_server); }
+    return b;
+}
+
+// sumsq of a group of `group` replicas cannot wrap u64: group * bound^2 < 2^64
+inline bool band_sumsq_fits(uint64_t group, uint64_t bound) {
+    return (unsigned __int128)group * bound * bound < ((unsigned __int128)1 << 64);
+}
 
 inline void make_layout(const AfScenario& s, const AfOptions& o, int32_t n_sweep_cols, afc::Layout& L) {
     L.n_edges = s.n_edges; L.n_servers = s.n_servers; L.n_endpoints = s.n_endpoints; L.n_steps = s.n_steps;

@@ -168,6 +168,13 @@ struct Cfg {
     const uint32_t* order;                          // the k-th replica a lane pulls is local index order[k] (af_run)
     const uint32_t* redo_list; const uint32_t* redo_count;
     uint64_t seed, replica_begin, n_replicas;
+    // per-tick bands (run_lane<true> only; DESIGN.md §3.4).  Group g's difference rows start at band_rows + g * band_group_words:
+    // row 0 counts replicas, rows 1 + j the sum of series j, rows 1 + n_series + j its square; band_stride words per row
+    // (ticks, plus one at index n_ticks for changes after the last tick).  A replica without a group entry adds to group
+    // band_groups, which is never fetched.
+    uint64_t* band_rows; const uint32_t* band_group; uint32_t* band_from;
+    uint64_t band_first, band_n, band_group_words;
+    int32_t band_groups, band_stride;
 };
 
 #if defined(__CUDACC__)
@@ -281,6 +288,7 @@ struct St {
     uint32_t completed, flags, traced;
     uint64_t n_events;
     double lat_sum, lat_sumsq, lat_min, lat_max;
+    uint64_t* band;                             // run_lane<true>: the replica's group's difference rows
 };
 
 // flags that end a replica early (its partial results are written back with the flag set)
@@ -531,8 +539,19 @@ AFL_IN bool gen_next_gap(St& W, double& gap) {
 // The accumulator and the maximum are only ever ADDED to / MAXED during the run and read at write-back: they live in
 // the lane's global tier and are updated with fire-and-forget reductions (no load, no wait, no shared memory: 12 B
 // per series -- on a 32-node topology 1.8 KB per lane, the difference between 2 and 6 warps per SM).
+//
+// Per-tick bands (kBands) ride on the same moment: a change from v to v + delta with n_ticks ticks taken before it adds
+// delta to the series at every tick k >= n_ticks, so the sums over a group's replicas are difference arrays -- one RED
+// of delta (and of (v + delta)^2 - v^2) at index n_ticks per change, one prefix scan after the launch (DESIGN.md §3.4).
+template <bool kBands>
 AFL_IN void gauge_touch(const St& W, const Mem& m, int32_t j, uint32_t v_old, int32_t delta) {
     red_add64(g64p(m, AFL_C.gi_acc + j), (uint64_t)(int64_t)delta * (uint64_t)W.n_ticks);
+    if constexpr (kBands) {
+        const uint64_t v1 = (uint64_t)(v_old + (uint32_t)delta), v0 = (uint64_t)v_old;
+        uint64_t* row = W.band + (uint64_t)(1 + j) * (uint64_t)AFL_C.band_stride + W.n_ticks;
+        red_add64(row, (uint64_t)(int64_t)delta);
+        red_add64(row + (uint64_t)AFL_C.n_series * (uint64_t)AFL_C.band_stride, v1 * v1 - v0 * v0);
+    }
     const int32_t dw = AFL_C.o32_dirty + (j >> 5);
     const uint32_t d = w32_ld(m, dw), bit = 1u << (j & 31);
     if (!(d & bit)) {
@@ -540,20 +559,22 @@ AFL_IN void gauge_touch(const St& W, const Mem& m, int32_t j, uint32_t v_old, in
         w32_st(m, dw, d | bit);
     }
 }
+template <bool kBands>
 AFL_IN void conn_add(const St& W, const Mem& m, uint32_t edge, int32_t delta) {
     const int32_t pw = AFL_C.o32_conn + (int32_t)edge;
     const uint32_t v = w32_ld(m, pw);
-    if (AFL_C.metrics_mask & AF_METRIC_EDGE_CONN) gauge_touch(W, m, 3 * AFL_C.n_servers + (int32_t)edge, v, delta);
+    if (AFL_C.metrics_mask & AF_METRIC_EDGE_CONN) gauge_touch<kBands>(W, m, 3 * AFL_C.n_servers + (int32_t)edge, v, delta);
     w32_st(m, pw, v + (uint32_t)delta);
 }
 AFL_IN int32_t ib_word(uint32_t node, int32_t f) { return AFL_C.c_inbox + (int32_t)node * IB_WORDS + f; }      // cold
 AFL_IN int32_t sq_word(uint32_t sidx, int32_t f) { return AFL_C.c_srvq + (int32_t)sidx * SQ_WORDS + f; }       // cold
 AFL_IN int32_t sv_word(uint32_t sidx, int32_t f) { return AFL_C.o32_srv + (int32_t)sidx * SV_WORDS + f; }
 // field = SV_READY_Q / SV_IO_Q / SV_RAM_IN_USE (series 3 * sidx + 0 / 1 / 2)
+template <bool kBands>
 AFL_IN void srv_gauge_add(const St& W, const Mem& m, uint32_t sidx, int32_t field, int32_t delta) {
     const int32_t pw = sv_word(sidx, field);
     const int32_t v = i32_ld(m, pw);
-    if ((AFL_C.metrics_mask & 7u) == 7u) gauge_touch(W, m, 3 * (int32_t)sidx + (field - SV_READY_Q), (uint32_t)v, delta);
+    if ((AFL_C.metrics_mask & 7u) == 7u) gauge_touch<kBands>(W, m, 3 * (int32_t)sidx + (field - SV_READY_Q), (uint32_t)v, delta);
     i32_st(m, pw, v + delta);
 }
 AFL_IN uint32_t gauge_value(const Mem& m, int32_t j) {
@@ -586,6 +607,31 @@ AFL_IN void take_ticks(St& W, const Mem& m, double t, uint32_t ev_seq) {
         for (int32_t w = 0; w < AFL_C.n_dirty; ++w) w32_st(m, AFL_C.o32_dirty + w, 0u);
     }
     W.tick_time = tick; W.tick_seq = tseq; W.n_ticks = nt; W.seq = seq;
+}
+
+// ---- per-tick bands: a replica joins its group's count at tick 0 (every gauge starts at 0), and a replica that a stop
+//      flag ends leaves at the tick it stopped at: its current values and its count are taken back there, so the
+//      frozen ticks to the horizon add nothing.  Every tick before n_ticks was taken before the event in which the
+//      flag was raised: those are exact, and the warp-per-replica pass re-runs the replica from that tick (band_from).
+AFL_IN void band_start(St& W) {
+    const uint64_t i = W.replica - AFL_C.band_first;
+    const uint32_t g = i < AFL_C.band_n ? AFL_C.band_group[i] : (uint32_t)AFL_C.band_groups;
+    W.band = AFL_C.band_rows + (uint64_t)g * AFL_C.band_group_words;
+    red_add64(W.band, 1u);
+}
+AFL_IN void band_stop(const St& W, const Mem& m) {
+    const uint64_t n = W.n_ticks, stride = (uint64_t)AFL_C.band_stride, sq = (uint64_t)AFL_C.n_series * stride;
+#pragma unroll 1
+    for (int32_t j = 0; j < AFL_C.n_series; ++j) {
+        if (!gauge_on(j)) continue;
+        const uint64_t v = gauge_value(m, j);
+        if (v == 0) continue;
+        uint64_t* row = W.band + (uint64_t)(1 + j) * stride + n;
+        red_add64(row, 0 - v);
+        red_add64(row + sq, 0 - v * v);
+    }
+    red_add64(W.band + n, ~0ull);
+    AFL_C.band_from[W.local] = (uint32_t)n;
 }
 
 // ---- Stores (mailboxes), Containers: as af_core.cuh ----------------------------------------------------
@@ -821,8 +867,10 @@ enum : uint32_t { A_NONE = 0, A_NODE, A_STEPS, A_SEND, A_TIMER };
 // The lane's life: pull a replica, run it to the horizon, write it back, pull the next.  `next_index`
 // returns the next local replica index or ~0 when the launch has no more work for this lane.
 // `converge` is a warp-wide rendez-vous at the top of every iteration (device: __any_sync).
+// `kBands`: also accumulate the per-tick bands of the replicas' groups (Cfg.band_*); false compiles to the same code
+// as before bands existed.
 // ---------------------------------------------------------------------------------------------------
-template <class NextFn, class ConvFn>
+template <bool kBands = false, class NextFn, class ConvFn>
 AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
     const Cfg& C = AFL_C;
     St W;
@@ -836,6 +884,7 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
             if (r == ~0ull) exhausted = true;
             else {
                 start_replica(W, m, r);
+                if constexpr (kBands) band_start(W);
                 // start order of the reference (simulation_runner.py:339-342, 301-336):
                 // spike timeline, outage timeline, generator, ..., collector
                 if (C.n_spike > 0) {
@@ -925,6 +974,7 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
         }
         AFL_SYNC();
         // ---- phase: collector ticks that fall before this event ------------------------------------------------
+        if constexpr (kBands) { if (AFL_UNLIKELY(dead)) band_stop(W, m); }     // before the frozen ticks to the horizon
         if (run && !is_item) {
             const double tick = W.tick_time;
             if (tick < t_ev || (tick == t_ev && W.tick_seq < ev_seq)) take_ticks(W, m, t_ev, ev_seq);
@@ -947,7 +997,7 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
         if (names_request) rq_load(W, m, slot, t0, rid, pack);
         if (is_event) {
             if (kind == K_DELIVER) {                          // edge.py:110-116: the edge's timeout fired
-                conn_add(W, m, aux, -1);
+                conn_add<kBands>(W, m, aux, -1);
                 const uint32_t meta = ro(C.edges + aux).meta;
                 pack += 1;                                     // record_hop(edge)
                 const uint32_t tk = (meta >> 3) & 3u;
@@ -994,11 +1044,11 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                 consumer_get(W, m, NODE_CLIENT);
             } else if (kind == I_RAM_OK) {                     // the RAM get event is processed: the handler resumes
                 sidx = aux;
-                srv_gauge_add(W, m, sidx, SV_RAM_IN_USE, (int32_t)ep_total_ram(m, pk_ep(pack)));
+                srv_gauge_add<kBands>(W, m, sidx, SV_RAM_IN_USE, (int32_t)ep_total_ram(m, pk_ep(pack)));
                 act = A_STEPS;
             } else if (kind == I_CPU_OK) {                     // the CPU get event is processed
                 sidx = aux;
-                if (pack & PK_WAIT) { pack &= ~PK_WAIT; srv_gauge_add(W, m, sidx, SV_READY_Q, -1); }
+                if (pack & PK_WAIT) { pack &= ~PK_WAIT; srv_gauge_add<kBands>(W, m, sidx, SV_READY_Q, -1); }
                 pack |= PK_CORE;
                 act = A_STEPS;
             } else if (kind == I_CPU_PUT) {                    // waiters are re-examined, then the request goes on
@@ -1045,7 +1095,7 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                         go = false;
                     } else {
                         i32_st(m, sv_word(sidx, SV_RAM_FREE), i32_ld(m, sv_word(sidx, SV_RAM_FREE)) - (int32_t)total_ram);   // granted, and its get event would run next
-                        srv_gauge_add(W, m, sidx, SV_RAM_IN_USE, (int32_t)total_ram);
+                        srv_gauge_add<kBands>(W, m, sidx, SV_RAM_IN_USE, (int32_t)total_ram);
                     }
                 }
                 if (go) act = A_STEPS;
@@ -1100,7 +1150,7 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                 if (st < ep.n_steps) {
                     const StepP sp = ro(C.steps + ep.step_begin + st);
                     if (sp.kind == AF_STEP_CPU) {
-                        if (pack & PK_IO) { pack &= ~PK_IO; srv_gauge_add(W, m, sidx, SV_IO_Q, -1); }
+                        if (pack & PK_IO) { pack &= ~PK_IO; srv_gauge_add<kBands>(W, m, sidx, SV_IO_Q, -1); }
                         if (!(pack & PK_CORE)) {             // cpu_req = CPU.get(1); yield cpu_req
                             if (can_fuse(W) && i32_ld(m, sv_word(sidx, SV_CPU_FREE)) > 0 && q_empty(W, m, sq_word(sidx, SQ_CPUQ_HEAD))) {
                                 i32_st(m, sv_word(sidx, SV_CPU_FREE), i32_ld(m, sv_word(sidx, SV_CPU_FREE)) - 1);     // granted, and its get event would run next
@@ -1108,7 +1158,7 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                             } else {
                                 fifo_push(m, sq_word(sidx, SQ_CPUQ_HEAD), sq_word(sidx, SQ_CPUQ_TAIL), slot);
                                 W.n_waiting += 1;
-                                if (!cpu_walk(W, m, sidx, slot)) { pack |= PK_WAIT; srv_gauge_add(W, m, sidx, SV_READY_Q, 1); }   // not cpu_req.triggered
+                                if (!cpu_walk(W, m, sidx, slot)) { pack |= PK_WAIT; srv_gauge_add<kBands>(W, m, sidx, SV_READY_Q, 1); }   // not cpu_req.triggered
                                 break;
                             }
                         }
@@ -1123,7 +1173,7 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                             nq_push(W, m, I_CPU_PUT, sidx, slot);
                             break;
                         }
-                        if (!(pack & PK_IO)) { pack |= PK_IO; srv_gauge_add(W, m, sidx, SV_IO_Q, 1); }
+                        if (!(pack & PK_IO)) { pack |= PK_IO; srv_gauge_add<kBands>(W, m, sidx, SV_IO_Q, 1); }
                     }
                     const double dur = sp.c_dur >= 0 ? row_val(m, sp.c_dur) : sp.dur;
                     tm_t = W.now + dur; tm_payload = mk_payload(K_STEP_END, sidx, slot); tm_seq = W.seq++;
@@ -1141,10 +1191,10 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                     nq_push(W, m, I_CPU_PUT, sidx, slot);
                     break;
                 }
-                if (pack & PK_IO) { pack &= ~PK_IO; srv_gauge_add(W, m, sidx, SV_IO_Q, -1); }
+                if (pack & PK_IO) { pack &= ~PK_IO; srv_gauge_add<kBands>(W, m, sidx, SV_IO_Q, -1); }
                 const uint32_t total_ram = ep.c_ram >= 0 ? (uint32_t)row_val(m, ep.c_ram) : ep.total_ram;
                 if (total_ram) {                             // yield RAM.put(total_ram): level rises NOW
-                    srv_gauge_add(W, m, sidx, SV_RAM_IN_USE, -(int32_t)total_ram);
+                    srv_gauge_add<kBands>(W, m, sidx, SV_RAM_IN_USE, -(int32_t)total_ram);
                     i32_st(m, sv_word(sidx, SV_RAM_FREE), i32_ld(m, sv_word(sidx, SV_RAM_FREE)) + (int32_t)total_ram);
                     if (!can_fuse(W)) { nq_push(W, m, I_RAM_PUT, sidx, slot); break; }
                     if (AFL_UNLIKELY(!q_empty(W, m, sq_word(sidx, SQ_RAMQ_HEAD)))) ram_walk(W, m, sidx);   // the put event would run next: waiters, then forward
@@ -1240,7 +1290,7 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                     rq_release(W, m, slot);
                 } else {
                     rq_pack_set(W, m, slot, pack);              // (the one store of the record on the request's way out of a node)
-                    conn_add(W, m, edge, 1);
+                    conn_add<kBands>(W, m, edge, 1);
                     double effective = transit;
                     if (C.n_spike > 0) effective = transit + f64_ld(m, C.o64_spike + (int32_t)edge);   // spike read at SEND time (edge.py:94-106)
                     else effective = transit + 0.0;         // (-0.0 + 0.0 = +0.0, as with a spike table of zeros)

@@ -32,6 +32,7 @@ class Engine:
         self._n = 0
         self._opt = K.AfOptions(0, 0, 0, 0, 1, 1, 0, 0)
         self._keep: list = []
+        self._band_groups = self._run_band_groups = 0
 
     # ------------------------------------------------------------------ plumbing
     def _check(self, rc: int, what: str) -> None:
@@ -89,6 +90,7 @@ class Engine:
     def run(self, seed: int, replica_begin: int, replica_end: int) -> None:
         self._check(self._lib.af_run(self._h, int(seed), int(replica_begin), int(replica_end)), "af_run")
         self._n = int(replica_end) - int(replica_begin)
+        self._run_band_groups = self._band_groups
 
     def sync(self) -> None:
         self._check(self._lib.af_sync(self._h), "af_sync")
@@ -155,6 +157,37 @@ class Engine:
         out = np.empty(K.AF_HIST_BINS, dtype=np.uint64)
         self._check(self._lib.af_reduce_histograms(self._h, out.ctypes.data), "af_reduce_histograms")
         return out
+
+    def upload_bands(self, groups: np.ndarray | None, first_replica: int = 0, n_groups: int | None = None) -> None:
+        """Per-tick bands from the next run on: ``groups[i]`` = group of replica ``first_replica + i`` (``None``: bands
+        off), ``n_groups`` groups (default: the largest group + 1) -- ``af_bands_upload``.  Replicas without an entry
+        contribute nothing."""
+        if groups is None:
+            self._check(self._lib.af_bands_upload(self._h, None, 0, 0, 0), "af_bands_upload")
+            self._band_groups = 0
+            return
+        g = np.ascontiguousarray(groups, dtype=np.uint32)
+        if n_groups is None:
+            n_groups = int(g.max()) + 1 if g.size else 0
+        self._check(self._lib.af_bands_upload(self._h, g.ctypes.data, g.size, int(first_replica), n_groups),
+                    "af_bands_upload")
+        self._band_groups = n_groups
+
+    def bands(self) -> tuple[np.ndarray, np.ndarray, np.ndarray]:
+        """Bands of the last run: ``(count [G, T] u32, sum [G, S, T] u64, sumsq [G, S, T] u64)`` -- per group, series
+        (the order of :meth:`sampled`) and tick, the replicas that contribute the tick, the sum of their values and
+        of their squares (``af_fetch_bands``)."""
+        flat = self.flat
+        cap = int(flat.horizon_s / flat.sample_period) + 2
+        G, S = self._run_band_groups, flat.n_series
+        count = np.empty((G, cap), dtype=np.uint32)
+        s = np.empty((G, S, cap), dtype=np.uint64)
+        sq = np.empty((G, S, cap), dtype=np.uint64)
+        n = C.c_uint64()
+        self._check(self._lib.af_fetch_bands(self._h, count.ctypes.data, s.ctypes.data, sq.ctypes.data, cap, C.byref(n)),
+                    "af_fetch_bands")
+        T = n.value
+        return count[:, :T].copy(), s[:, :, :T].copy(), sq[:, :, :T].copy()
 
     def trace_clocks(self, local_replica: int) -> np.ndarray:
         cap = max(1, self._opt.trace_clock_capacity)

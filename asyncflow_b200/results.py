@@ -182,6 +182,11 @@ class SweepResults:
         self.rows: np.ndarray | None = None      # sweep row of each result row (set by SweepRunner)
         self.traced: list[ReplicaResults] = []    # full clocks + sampled series of the first `trace_replicas` replica ids
         self.exact: np.ndarray | None = None      # rows whose p50/p95/p99 are exact (SweepRunner.exact_percentiles)
+        # per-tick bands (SweepRunner(bands=...)): per group g, series j, tick k: replicas that contribute the tick,
+        # sum of their values, sum of the squares -- [G, T] u32, [G, n_series, T] u64, [G, n_series, T] u64
+        self.band_count: np.ndarray | None = None
+        self.band_sum: np.ndarray | None = None
+        self.band_sumsq: np.ndarray | None = None
 
     def __len__(self) -> int:
         return int(self.stats.shape[0])
@@ -274,18 +279,66 @@ class SweepResults:
                            self.samp_sum[index], self.samp_max[index], g(self.throughput), g(self.histograms),
                            self.replica_begin)
         out.traced = self.traced
+        out.band_count, out.band_sum, out.band_sumsq = self.band_count, self.band_sum, self.band_sumsq
         return out
 
     def bands(self, key: Any, entity_id: str) -> dict[str, np.ndarray]:
         """``series_bands`` over this sweep's traced replicas (``SweepRunner(trace_replicas=k)``)."""
         return series_bands(self.traced, key, entity_id)
 
+    def series_index(self, key: Any, entity_id: str) -> int | None:
+        """Row of ``(key, entity_id)`` -- as ``ResultsAnalyzer.get_series`` takes them -- in the sampled series, or
+        ``None`` when the scenario does not sample that metric."""
+        name = str(getattr(key, "value", key))
+        en = set(self.flat.enabled_metrics)
+        if name in SERVER_SERIES:
+            i = list(self.flat.server_ids).index(entity_id)
+            return 3 * i + SERVER_SERIES.index(name) if all(m in en for m in SERVER_SERIES) else None
+        if name == EDGE_SERIES:
+            e = list(self.flat.edge_ids).index(entity_id)
+            return 3 * self.flat.n_servers + e if EDGE_SERIES in en else None
+        msg = f"unknown sampled metric {name!r}"
+        raise KeyError(msg)
+
+    def group_bands(self, key: Any, entity_id: str, level: float = 0.95) -> dict[str, np.ndarray]:
+        """Per group and tick, over the group's replicas, of one sampled series (``SweepRunner(bands=...)``):
+        ``{"t", "n", "mean", "std", "lo", "hi"}``, each ``[G, T]`` but ``t`` (``[T]``, seconds).  ``t[k] = k *
+        sample_period``, the time axis ``get_series`` gives the same samples (so a band overlays a traced replica's
+        curve); the collector takes tick ``k`` at simulated time ``(k + 1) * sample_period``.  ``std`` has
+        ddof = 1 and ``lo`` / ``hi`` are a normal ``level`` interval on the mean, as in :meth:`confidence_interval`;
+        NaN where fewer than two replicas contribute the tick.  ``key`` / ``entity_id`` as in
+        ``ResultsAnalyzer.get_series`` (``metrics/analyzer.py:239-262``), lifted from one replica to a sweep."""
+        if self.band_count is None:
+            msg = "no bands: run the sweep with SweepRunner(bands=...)"
+            raise ValueError(msg)
+        j = self.series_index(key, entity_id)
+        G, T = self.band_count.shape
+        if j is None:
+            z = np.zeros((G, 0))
+            return {"t": np.zeros(0), "n": self.band_count[:, :0], "mean": z, "std": z, "lo": z, "hi": z}
+        n = self.band_count.astype(np.float64)
+        s = self.band_sum[:, j, :].astype(np.float64)
+        sq = self.band_sumsq[:, j, :].astype(np.float64)
+        with np.errstate(invalid="ignore", divide="ignore"):
+            mean = np.where(n > 0, s / n, np.nan)
+            var = np.where(n > 1, np.maximum(sq - s * mean, 0.0) / (n - 1.0), np.nan)
+            std = np.sqrt(var)
+            from statistics import NormalDist  # noqa: PLC0415
+            half = NormalDist().inv_cdf(0.5 + level / 2.0) * std / np.sqrt(n)
+        return {"t": np.arange(T) * self.flat.sample_period, "n": self.band_count, "mean": mean, "std": std,
+                "lo": mean - half, "hi": mean + half}
+
     @staticmethod
     def concatenate(parts: list["SweepResults"]) -> "SweepResults":
         f = parts[0]
         cat = lambda xs: None if xs[0] is None else np.concatenate(xs)  # noqa: E731
-        return SweepResults(
+        out = SweepResults(
             f.flat, np.concatenate([p.stats for p in parts]), np.concatenate([p.edge_sent for p in parts]),
             np.concatenate([p.edge_dropped for p in parts]), np.concatenate([p.samp_sum for p in parts]),
             np.concatenate([p.samp_max for p in parts]), cat([p.throughput for p in parts]),
             cat([p.histograms for p in parts]), f.replica_begin)
+        if all(p.band_count is not None for p in parts):      # integer sums over disjoint replicas: they add exactly
+            out.band_count = np.sum([p.band_count for p in parts], axis=0, dtype=np.uint32)
+            out.band_sum = np.sum([p.band_sum for p in parts], axis=0, dtype=np.uint64)
+            out.band_sumsq = np.sum([p.band_sumsq for p in parts], axis=0, dtype=np.uint64)
+        return out

@@ -38,7 +38,7 @@
 extern "C" {
 #endif
 
-#define AF_ABI_VERSION 2
+#define AF_ABI_VERSION 3
 
 typedef enum AfStatus {
     AF_OK = 0,
@@ -257,6 +257,26 @@ int af_fetch_trace_clocks(af_engine* e, uint64_t local_replica, double* start_fi
                           uint64_t capacity_pairs, uint64_t* n_pairs);
 int af_fetch_trace_series(af_engine* e, uint64_t local_replica, uint32_t* values,
                           uint64_t capacity_ticks, uint64_t* n_ticks); /* [series][capacity_ticks] */
+
+/* Per-tick sampled-metric bands over groups of replicas, accumulated on the device.
+ * group_of[i] = group (< n_groups) of replica first_replica + i; NULL clears (bands off).  Every later af_run then
+ * sums, for every group g, series j (the order of af_fetch_sampled) and tick k < n_ticks (the ticks a replica that
+ * reaches the horizon takes):
+ *   count[g][k]     replicas of g that contribute tick k
+ *   sum[g][j][k]    sum of their values of series j at tick k (the value a traced replica stores at tick k)
+ *   sumsq[g][j][k]  sum of the squares
+ * A replica contributes every tick it took before a stop flag ended it; a replica the thread-per-replica pass flags
+ * and the warp-per-replica pass re-runs inside the same af_run contributes once, in full.  Replicas without a group
+ * entry contribute nothing.  Every other output is the same with bands on or off.  Rejected (AF_ERR_INVALID) when
+ * group size x (bound on a gauge)^2 could wrap the u64 sums of squares (the bound is the request capacity or the
+ * largest ram_mb, swept values included), when the scenario takes 5e7 ticks or more, or when the band rows,
+ * (n_groups + 1) x (1 + 2 n_series) x (n_ticks + 1) x 8 bytes, exceed the device's memory; af_run checks all of it
+ * again with the scenario, options and sweep of the run. */
+int af_bands_upload(af_engine* e, const uint32_t* group_of, uint64_t n, uint64_t first_replica, uint32_t n_groups);
+/* bands of the last af_run: count[g][k], sum[g][j][k], sumsq[g][j][k], k < min(*n_ticks, capacity_ticks), rows of
+ * capacity_ticks entries; *n_ticks = the run's tick count.  Any of the three arrays may be NULL (not fetched). */
+int af_fetch_bands(af_engine* e, uint32_t* count, uint64_t* sum, uint64_t* sumsq,
+                   uint64_t capacity_ticks, uint64_t* n_ticks);
 
 /* AF-RNG known-answer hook: the device's random numbers outside the state machine, n values per call
  * (the streams of oracle/afrng.py; tests/test_gpu_rng.py compares them bit for bit with oracle/afrng_c):
