@@ -11,7 +11,7 @@ from __future__ import annotations
 import ctypes as C
 from pathlib import Path
 
-AF_ABI_VERSION = 3
+AF_ABI_VERSION = 4
 AF_HIST_BINS = 4096
 AF_HIST_SUB_BITS = 7
 AF_HIST_MIN_EXP = -20
@@ -119,6 +119,10 @@ class AfRunPasses(C.Structure):
                 ("lane_replicas", C.c_uint64), ("warp_replicas", C.c_uint64), ("lane_pool_elems", C.c_int32)]
 
 
+class AfBandOptions(C.Structure):
+    _fields_ = [("sampled", C.c_int32), ("latency_window_s", C.c_int32)]
+
+
 class EngineUnavailable(RuntimeError):
     """The CUDA engine cannot run here (library not built or no usable GPU)."""
 
@@ -131,7 +135,7 @@ EXPORTS = [
     "af_last_run_ms", "af_launch_count", "af_fetch_stats", "af_fetch_edge_counts",
     "af_fetch_histograms", "af_fetch_throughput", "af_fetch_sampled", "af_fetch_trace_clocks",
     "af_fetch_trace_series", "af_reduce_histograms", "af_engine_set_mode", "af_last_run_passes",
-    "af_selftest_rng", "af_bands_upload", "af_fetch_bands",
+    "af_selftest_rng", "af_bands_upload", "af_fetch_bands", "af_bands_configure", "af_fetch_latency_bands",
 ]
 
 _lib = None
@@ -177,6 +181,8 @@ def load() -> C.CDLL:
     lib.af_selftest_rng.argtypes = [vp, u64, u64, i32, i32, C.c_double, C.c_double, C.c_uint32, u64, vp, vp]
     lib.af_bands_upload.argtypes = [vp, vp, u64, u64, C.c_uint32]
     lib.af_fetch_bands.argtypes = [vp, vp, vp, vp, u64, C.POINTER(u64)]
+    lib.af_bands_configure.argtypes = [vp, C.POINTER(AfBandOptions)]
+    lib.af_fetch_latency_bands.argtypes = [vp, vp, vp, vp, u64, C.POINTER(u64)]
     for name in EXPORTS:
         fn = getattr(lib, name)
         if fn.restype is C.c_int and name not in ("af_abi_version",):

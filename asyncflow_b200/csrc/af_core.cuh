@@ -176,6 +176,10 @@ struct State {
     // words per difference row, the byte offset of the table of each series' last emitted value (u32, behind the tables)
     uint64_t* band;
     uint32_t band_from, band_stride, band_prev_off, band_pad;
+    // per-window latency bands: the replica's group's windows (nullptr: off), the completions the thread-per-replica
+    // pass already added (a re-run adds from there on), the window width in seconds
+    uint64_t* lat;
+    uint32_t lat_from, lat_window;
 };
 
 // Everything the kernel needs to know about sizes; built on the host.
@@ -201,10 +205,14 @@ struct Layout {
 // group g's difference rows start at rows + g * group_words; from[local] = the tick from which a re-run of a flagged
 // replica contributes (the thread-per-replica pass contributed the ticks before it); prev_off = byte offset of the
 // table of each series' last emitted value in the warp's workspace (4 * n_series bytes behind Layout.warp_bytes).
+// Per-window latency bands (lat_window == 0: off), over the same groups: group g's windows start at
+// lat_rows + g * lat_windows * afr::LAT_ROW; lat_from[local] = the completions the thread-per-replica pass added.
 struct BandArgs {
     uint64_t* rows; const uint32_t* group; const uint32_t* from;
     uint64_t first, n, group_words;
     uint32_t groups, stride; int32_t prev_off, pad;
+    uint64_t* lat_rows; const uint32_t* lat_from;
+    uint32_t lat_window, lat_windows;
 };
 
 constexpr int32_t NQ_CAP = 128;   // now-queue capacity (power of two)
@@ -725,6 +733,19 @@ AF_IN void server_got(State& W, uint32_t slot, uint32_t sidx, const ReqRec& r) {
 // ---------------------------------------------------------------------------------
 // client: completion (client.py:62-69 + analyzer.py:83-125)
 // ---------------------------------------------------------------------------------
+// per-window latency bands: one to the latency's bin and the latency in 32.32 fixed point to the two sum words of the
+// finish window (af_lane.cuh's lat_add; the caller has checked that this completion counts)
+AF_IN void lat_add(const State& W, double now, double lat) {
+    int32_t b = (int32_t)ceil(now) - 1;
+    b = b < 0 ? 0 : b;
+    if (b >= AF_L.horizon_s) return;
+    uint64_t* row = W.lat + (uint64_t)((uint32_t)b / W.lat_window) * afr::LAT_ROW;
+    red_add_u64(row + afr::hist_bin(lat), 1u);
+    const uint64_t u = afr::lat_fixed32(lat);
+    if (u >> 32) red_add_u64(row + AF_HIST_BINS, u >> 32);
+    red_add_u64(row + AF_HIST_BINS + 1, u & 0xFFFFFFFFull);
+}
+
 AF_IN void complete(State& W, uint32_t slot, double t0) {
     const double now = W.now;
     const double lat = now - t0;                     // finish - start (analyzer.py:86-89)
@@ -737,12 +758,10 @@ AF_IN void complete(State& W, uint32_t slot, double t0) {
     if (traced && (int32_t)(done - 1) >= AF_L.trace_clock_cap) W.flags |= AF_FLAG_TRACE_TRUNCATED;
     if (lane_id() == 0) {
         const uint64_t local = W.local;
-        if (AF_L.collect_hist) {
-            int32_t idx = (int32_t)(afr::d2u(lat) >> (52 - AF_HIST_SUB_BITS))
-                          - ((1023 + AF_HIST_MIN_EXP) << AF_HIST_SUB_BITS);
-            idx = idx < 0 ? 0 : (idx >= AF_HIST_BINS ? AF_HIST_BINS - 1 : idx);
-            red_add_u32(&AF_G.hist[local * AF_HIST_BINS + (uint32_t)idx], 1u);
-        }
+        if (AF_L.collect_hist) red_add_u32(&AF_G.hist[local * AF_HIST_BINS + (uint32_t)afr::hist_bin(lat)], 1u);
+        // a completion counts in the latency bands while no stop flag is set (what follows a flag may differ from a
+        // re-run), and in a re-run only from the first one the thread-per-replica pass did not add
+        if (W.lat != nullptr && done > W.lat_from && !(W.flags & STOP_FLAGS)) lat_add(W, now, lat);
         if (AF_L.collect_thr) {
             // bucket k counts (k, k+1] (analyzer.py:108-125)
             int32_t b = (int32_t)ceil(now) - 1;
@@ -1138,11 +1157,18 @@ AF_IN void run_replica(State& W, uint64_t local_index, const BandArgs& band) {
     W.lat_sum = 0.0; W.lat_sumsq = 0.0; W.lat_min = afr::u2d(INF_BITS); W.lat_max = 0.0;
     W.traced = (int64_t)local_index < (int64_t)AF_L.trace_replicas ? 1u : 0u;
     W.band = nullptr; W.band_from = 0; W.band_stride = band.stride; W.band_prev_off = (uint32_t)band.prev_off;
-    if (band.stride) {
+    W.lat = nullptr; W.lat_from = 0; W.lat_window = band.lat_window;
+    if (band.stride || band.lat_window) {
         const uint64_t i = W.replica - band.first;
         const uint32_t g = i < band.n ? band.group[i] : band.groups;
-        W.band = band.rows + (uint64_t)g * band.group_words;
-        W.band_from = AF_G.redo_list ? band.from[local_index] : 0u;      // a re-run continues where the lane pass stopped
+        if (band.stride) {
+            W.band = band.rows + (uint64_t)g * band.group_words;
+            W.band_from = AF_G.redo_list ? band.from[local_index] : 0u;  // a re-run continues where the lane pass stopped
+        }
+        if (band.lat_window) {
+            W.lat = band.lat_rows + (uint64_t)g * band.lat_windows * afr::LAT_ROW;
+            W.lat_from = AF_G.redo_list ? band.lat_from[local_index] : 0u;
+        }
     }
     w_sync();
     load_params(W);

@@ -15,6 +15,7 @@
 //                         persistent CTAs pulling replica indices from a global counter; per-warp workspace in
 //                         shared memory with spill tiers in HBM.
 //   af_band_scan_kernel   per-tick bands (af_bands_upload): the groups' difference rows -> per-tick sums, in place
+//                         (per-window latency bands need no pass after the kernels: their rows are the sums)
 //   af_percentile_kernel  HBM-bound pass over the per-replica latency histograms:
 //                         one warp per replica, coalesced 128-byte row reads, warp
 //                         prefix sums, numpy-"linear" p50/p95/p99.
@@ -86,12 +87,13 @@ __global__ void AF_LAUNCH_BOUNDS af_sim_kernel(const afc::BandArgs band) {
 
 // One replica per thread.  Compiled for one CTA of up to 384 threads per SM (the shared-memory budget of a
 // lane decides the CTA size at launch).  More warps shrink each lane's share of shared memory (more of the heap lives
-// in L2), so the register budget is spent at 12 warps: 158 registers on sm_90a, no spills.  kBands: the same kernel
-// also accumulating per-tick bands (af_run uses it when groups are uploaded); <false> is the kernel without them.
+// in L2), so the register budget is spent at 12 warps: 158 registers on sm_90a, no spills.  kSampled / kLatency: the
+// same kernel also accumulating the per-tick / per-window latency bands of the uploaded groups (af_run picks the one
+// the band options ask for); <false, false> is the kernel without them.
 #ifndef AF_LANE_MAX_THREADS
 #define AF_LANE_MAX_THREADS 384
 #endif
-template <bool kBands = false>
+template <bool kSampled = false, bool kLatency = false>
 __global__ void __launch_bounds__(AF_LANE_MAX_THREADS, 1) af_lane_kernel() {
     const afl::Cfg& C = afl::c_cfg;
     const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
@@ -104,7 +106,7 @@ __global__ void __launch_bounds__(AF_LANE_MAX_THREADS, 1) af_lane_kernel() {
     m.g128 = gs + lane * 16u;
     m.g64 = gs + (size_t)C.gn128 * afl::STRIDE128 + lane * 8u;
     m.g32 = gs + (size_t)C.gn128 * afl::STRIDE128 + (size_t)C.gn64 * afl::STRIDE64 + lane * 4u;
-    afl::run_lane<kBands>(m,
+    afl::run_lane<kSampled, kLatency>(m,
         [&]() -> uint64_t {
             const unsigned long long k = atomicAdd(C.work_counter, 1ull);
             return k < C.n_replicas ? (uint64_t)C.order[k] : ~0ull;
@@ -369,6 +371,11 @@ struct af_engine {
     DevBuf d_band_group, d_band, d_band_from;
     uint64_t band_swept_ram = 0; int32_t band_swept_server = -1;     // afh::swept_ram_max of the uploaded sweep
     bool last_bands = false; uint32_t last_band_groups = 0, last_band_ticks = 0; uint64_t last_band_stride = 0;
+    // af_bands_configure: per-tick bands on (default) / off; per-window latency bands of lat_window seconds (0: off) --
+    // their rows, the completions each flagged replica added in the thread-per-replica pass
+    int32_t band_sampled = 1, lat_window = 0;
+    DevBuf d_lat, d_lat_from;
+    bool last_lat = false; uint32_t last_lat_groups = 0; uint64_t last_lat_windows = 0;
 
     int fail(int code, const std::string& m) { err = m; return code; }
     int cuda_fail(cudaError_t e, const char* what) {
@@ -442,7 +449,7 @@ void af_engine_destroy(af_engine* e) {
                       &e->d_stats, &e->d_sent, &e->d_dropped, &e->d_hist, &e->d_thr, &e->d_ssum, &e->d_smax,
                       &e->d_tclk, &e->d_tser, &e->d_tcnt, &e->d_counter, &e->d_htot,
                       &e->d_okey, &e->d_oidx, &e->d_order, &e->d_okey64, &e->d_sort_tmp,
-                      &e->d_band_group, &e->d_band, &e->d_band_from};
+                      &e->d_band_group, &e->d_band, &e->d_band_from, &e->d_lat, &e->d_lat_from};
     for (DevBuf* b : bufs) b->release();
     cudaEventDestroy(e->ev_begin); cudaEventDestroy(e->ev_sim); cudaEventDestroy(e->ev_end);
     cudaStreamDestroy(e->stream);
@@ -593,6 +600,32 @@ static uint64_t largest_group(const uint32_t* group_of, uint64_t n) {
     return best;
 }
 
+// the latency bands' window and rows for `n_groups` groups of the current scenario (afh::lat_bands_fit)
+static int lat_check(af_engine* e, uint64_t n_groups) {
+    std::string why;
+    if (!afh::lat_bands_fit(e->lat_window, e->sc.horizon_s, n_groups, e->mem_total, why)) return e->fail(AF_ERR_INVALID, why);
+    return AF_OK;
+}
+
+int af_bands_configure(af_engine* e, const AfBandOptions* opt) {
+    if (!e || !opt) return AF_ERR_INVALID;
+    if (opt->latency_window_s != 0) {
+        std::string why;
+        if (!afh::lat_bands_fit(opt->latency_window_s, 0, 0, e->mem_total, why)) return e->fail(AF_ERR_INVALID, why);
+    }
+    const int32_t sampled = e->band_sampled, window = e->lat_window;
+    e->band_sampled = opt->sampled != 0; e->lat_window = opt->latency_window_s;
+    int rc = AF_OK;
+    if (e->have_scenario && e->band_groups > 0) {        // the uploaded groups, under the new options
+        uint32_t ticks = 0;
+        if (e->band_sampled && !(rc = band_shape_check(e, e->band_groups, ticks)))
+            rc = band_check(e, largest_group(e->h_band_group.data(), e->h_band_group.size()));
+        if (!rc && e->lat_window) rc = lat_check(e, e->band_groups);
+    }
+    if (rc) { e->band_sampled = sampled; e->lat_window = window; }
+    return rc;
+}
+
 int af_bands_upload(af_engine* e, const uint32_t* group_of, uint64_t n, uint64_t first_replica, uint32_t n_groups) {
     if (!e) return AF_ERR_INVALID;
     if (!e->have_scenario) return e->fail(AF_ERR_STATE, "af_bands_upload before af_scenario_upload");
@@ -606,9 +639,12 @@ int af_bands_upload(af_engine* e, const uint32_t* group_of, uint64_t n, uint64_t
             return e->fail(AF_ERR_INVALID, b);
         }
     uint32_t ticks = 0;
-    int rc = band_shape_check(e, n_groups, ticks);
-    if (rc) return rc;
-    if ((rc = band_check(e, largest_group(group_of, n)))) return rc;
+    int rc;
+    if (e->band_sampled) {
+        if ((rc = band_shape_check(e, n_groups, ticks))) return rc;
+        if ((rc = band_check(e, largest_group(group_of, n)))) return rc;
+    }
+    if (e->lat_window && (rc = lat_check(e, n_groups))) return rc;
     e->h_band_group.assign(group_of, group_of + n);
     if ((rc = upload_vec(e, e->d_band_group, e->h_band_group, "band groups"))) return rc;
     AF_CUDA(e, cudaStreamSynchronize(e->stream), "band groups H2D");
@@ -701,7 +737,7 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
     afh::make_layout(e->sc, e->opt, e->sweep_cols, L);
 
     // ---- per-tick bands: difference rows of (groups + 1) x (1 + 2 n_series) x (ticks + 1) words -----------------------
-    const bool bands = e->band_groups > 0;
+    const bool bands = e->band_groups > 0 && e->band_sampled;
     uint32_t ticks32 = 0;
     if (bands) {      // (the scenario, options and sweep may have changed since af_bands_upload)
         if ((rc = band_shape_check(e, e->band_groups, ticks32))) return rc;
@@ -717,6 +753,11 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
         band.prev_off = L.warp_bytes;                       // the warp engine: each series' last emitted value, behind its tables
         L.warp_bytes += afc::align_up(4 * L.n_series, 16);
     }
+    // ---- per-window latency bands: (groups + 1) x windows x afr::LAT_ROW words ---------------------------------------------
+    const bool lat = e->band_groups > 0 && e->lat_window > 0;
+    if (lat && (rc = lat_check(e, e->band_groups))) return rc;
+    const uint64_t lat_windows = lat ? afh::lat_windows(L.horizon_s, e->lat_window) : 0;
+    const uint64_t lat_words = lat ? ((uint64_t)e->band_groups + 1) * lat_windows * afr::LAT_ROW : 0;
 
     // ---- launch shapes -------------------------------------------------------------------------------------
     // warp-per-replica: persistent CTAs of <= 4 warps (__launch_bounds__(128, AF_MIN_BLOCKS)), as many per SM as fit
@@ -739,7 +780,8 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
     }
     // thread-per-replica: one persistent CTA per SM
     uint64_t lgrid = 0; size_t lsmem = 0;
-    void (*lane_kernel)() = bands ? af_lane_kernel<true> : af_lane_kernel<false>;
+    void (*lane_kernel)() = bands ? (lat ? af_lane_kernel<true, true> : af_lane_kernel<true, false>)
+                                  : (lat ? af_lane_kernel<false, true> : af_lane_kernel<false, false>);
     if (lane) {
         lsmem = (size_t)lane_warps * (size_t)C.warp_bytes;
         AF_CUDA(e, cudaFuncSetAttribute(lane_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lsmem), "smem attribute");
@@ -789,6 +831,10 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
         AF_CUDA(e, e->d_band.ensure(band_words * 8), "band rows");
         AF_CUDA(e, e->d_band_from.ensure(n * 4), "band stop ticks");
     }
+    if (lat) {
+        AF_CUDA(e, e->d_lat.ensure(lat_words * 8), "latency band rows");
+        AF_CUDA(e, e->d_lat_from.ensure(n * 4), "latency band completions");
+    }
     // pull order: the first pass runs `workers` replicas at once (lanes, or warps without the thread-per-replica pass)
     const uint64_t workers = lane ? lgrid * (uint64_t)lane_warps * 32ull : warp_slots;
     const uint64_t wave = workers < n ? workers : n;
@@ -831,10 +877,14 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
     G.redo_list = redo ? (const uint32_t*)e->d_redo_list.p : nullptr;
     G.redo_count = redo ? (const uint32_t*)e->d_redo_count.p : nullptr;
     G.seed = seed; G.replica_begin = begin; G.n_replicas = n;
+    if (bands || lat) { band.group = (const uint32_t*)e->d_band_group.p; band.first = e->band_first; band.n = e->h_band_group.size(); band.groups = e->band_groups; }
     if (bands) {
-        band.rows = (uint64_t*)e->d_band.p; band.group = (const uint32_t*)e->d_band_group.p; band.from = (const uint32_t*)e->d_band_from.p;
-        band.first = e->band_first; band.n = e->h_band_group.size(); band.group_words = band_group_words;
-        band.groups = e->band_groups; band.stride = (uint32_t)band_stride;
+        band.rows = (uint64_t*)e->d_band.p; band.from = (const uint32_t*)e->d_band_from.p;
+        band.group_words = band_group_words; band.stride = (uint32_t)band_stride;
+    }
+    if (lat) {
+        band.lat_rows = (uint64_t*)e->d_lat.p; band.lat_from = (const uint32_t*)e->d_lat_from.p;
+        band.lat_window = (uint32_t)e->lat_window; band.lat_windows = (uint32_t)lat_windows;
     }
     if (lane) {
         C.edges = (const afl::EdgeP*)e->d_l_edges.p; C.servers = (const afl::ServerP*)e->d_l_servers.p;
@@ -850,10 +900,14 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
         C.work_counter = (unsigned long long*)e->d_counter2.p;
         C.order = G.order;
         C.seed = seed; C.replica_begin = begin; C.n_replicas = n;
+        if (bands || lat) { C.band_group = band.group; C.band_first = band.first; C.band_n = band.n; C.band_groups = (int32_t)e->band_groups; }
         if (bands) {
-            C.band_rows = band.rows; C.band_group = band.group; C.band_from = (uint32_t*)e->d_band_from.p;
-            C.band_first = band.first; C.band_n = band.n; C.band_group_words = band_group_words;
-            C.band_groups = (int32_t)e->band_groups; C.band_stride = (int32_t)band_stride;
+            C.band_rows = band.rows; C.band_from = (uint32_t*)e->d_band_from.p;
+            C.band_group_words = band_group_words; C.band_stride = (int32_t)band_stride;
+        }
+        if (lat) {
+            C.lat_rows = band.lat_rows; C.lat_from = (uint32_t*)e->d_lat_from.p;
+            C.lat_window = e->lat_window; C.lat_windows = (int32_t)lat_windows;
         }
     }
 
@@ -871,6 +925,7 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
     if (L.collect_hist) AF_CUDA(e, cudaMemsetAsync(e->d_hist.p, 0, n * AF_HIST_BINS * 4, e->stream), "memset hist");
     if (L.collect_thr) AF_CUDA(e, cudaMemsetAsync(e->d_thr.p, 0, n * (uint64_t)L.horizon_s * 4, e->stream), "memset thr");
     if (bands) AF_CUDA(e, cudaMemsetAsync(e->d_band.p, 0, band_words * 8, e->stream), "memset band rows");
+    if (lat) AF_CUDA(e, cudaMemsetAsync(e->d_lat.p, 0, lat_words * 8, e->stream), "memset latency band rows");
     {   // the pull order: (work, local index) heaviest first; then the first wave grouped by estimate
         uint32_t* key = (uint32_t*)e->d_okey.p; uint32_t* idx = (uint32_t*)e->d_oidx.p; uint32_t* order = (uint32_t*)e->d_order.p;
         uint64_t* key64 = (uint64_t*)e->d_okey64.p;
@@ -924,6 +979,7 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
     e->last_lane = lane; e->last_warp = warp; e->last_lane_warps = lane_warps;
     e->last_bands = bands; e->last_band_groups = e->band_groups; e->last_band_ticks = (uint32_t)band_ticks;
     e->last_band_stride = band_stride;
+    e->last_lat = lat; e->last_lat_groups = e->band_groups; e->last_lat_windows = lat_windows;
     return AF_OK;
 }
 
@@ -1096,6 +1152,28 @@ int af_fetch_bands(af_engine* e, uint32_t* count, uint64_t* sum, uint64_t* sumsq
         for (uint64_t g = 0; g < G; ++g)
             for (uint64_t t = 0; t < k; ++t) count[g * cap_ticks + t] = (uint32_t)c64[g * k + t];
     return AF_OK;
+}
+
+int af_fetch_latency_bands(af_engine* e, uint64_t* hist, uint64_t* sum_hi, uint64_t* sum_lo, uint64_t cap_windows,
+                           uint64_t* n_windows) {
+    if (!e || !n_windows) return AF_ERR_INVALID;
+    if (!e->ran) return e->fail(AF_ERR_STATE, "fetch before af_run");
+    if (!e->last_lat) return e->fail(AF_ERR_STATE, "the last run collected no latency bands (af_bands_configure, af_bands_upload)");
+    AF_CUDA(e, cudaSetDevice(e->device), "cudaSetDevice");
+    const uint64_t W = e->last_lat_windows, G = e->last_lat_groups, R = afr::LAT_ROW, B = AF_HIST_BINS;
+    const uint64_t k = W < cap_windows ? W : cap_windows;
+    *n_windows = W;
+    const uint64_t* base = (const uint64_t*)e->d_lat.p;
+    for (uint64_t g = 0; g < G && k; ++g) {                // window j of group g: row g * W + j
+        const uint64_t* gb = base + g * W * R;
+        if (hist) AF_CUDA(e, cudaMemcpy2DAsync(hist + g * cap_windows * B, B * 8, gb, R * 8, B * 8, k, cudaMemcpyDeviceToHost, e->stream),
+                          "latency band histograms D2H");
+        if (sum_hi) AF_CUDA(e, cudaMemcpy2DAsync(sum_hi + g * cap_windows, 8, gb + B, R * 8, 8, k, cudaMemcpyDeviceToHost, e->stream),
+                            "latency band sums D2H");
+        if (sum_lo) AF_CUDA(e, cudaMemcpy2DAsync(sum_lo + g * cap_windows, 8, gb + B + 1, R * 8, 8, k, cudaMemcpyDeviceToHost, e->stream),
+                            "latency band sums D2H");
+    }
+    return af_sync(e);
 }
 
 int af_fetch_trace_series(af_engine* e, uint64_t local, uint32_t* out, uint64_t cap_ticks, uint64_t* n_ticks) {

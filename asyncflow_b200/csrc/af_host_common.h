@@ -105,6 +105,31 @@ inline unsigned __int128 band_row_bytes(uint64_t n_groups, int32_t n_series, uin
     return ((unsigned __int128)n_groups + 1) * (unsigned __int128)(1 + 2 * (uint64_t)n_series) * ((unsigned __int128)ticks + 1) * 8u;
 }
 
+// Per-window latency bands: ceil(horizon / window) windows of `window_s` seconds, the last one cut at the horizon.
+inline uint64_t lat_windows(int32_t horizon_s, int32_t window_s) {
+    return ((uint64_t)(horizon_s > 0 ? horizon_s : 0) + (uint64_t)window_s - 1) / (uint64_t)window_s;
+}
+// bytes of the windows of n_groups groups plus the one of the replicas without a group
+inline unsigned __int128 lat_row_bytes(uint64_t n_groups, uint64_t windows) {
+    return ((unsigned __int128)n_groups + 1) * (unsigned __int128)windows * afr::LAT_ROW * 8u;
+}
+// The checks af_bands_configure, af_bands_upload and af_run apply to latency bands of `window_s` seconds over n_groups
+// groups: a positive window, and rows the device (mem_total bytes) can hold.
+inline bool lat_bands_fit(int32_t window_s, int32_t horizon_s, uint64_t n_groups, uint64_t mem_total, std::string& why) {
+    if (window_s < 1) {
+        why = "latency bands: window of " + std::to_string(window_s) + " s; the width is a whole number of seconds >= 1";
+        return false;
+    }
+    const uint64_t w = lat_windows(horizon_s, window_s);
+    const unsigned __int128 bytes = lat_row_bytes(n_groups, w);
+    if (bytes <= (unsigned __int128)mem_total) return true;
+    char b[256];
+    snprintf(b, sizeof b, "latency bands: %llu groups x %llu windows of %d s need %.3g GB of rows, more than the device's %.3g GB",
+             (unsigned long long)n_groups, (unsigned long long)w, window_s, (double)bytes / 1e9, (double)mem_total / 1e9);
+    why = b;
+    return false;
+}
+
 // The largest ram_mb a sweep sets (0: none), and the server it belongs to.
 inline uint64_t swept_ram_max(const AfSweepColumn* cols, int32_t n_cols, const double* vals, uint64_t n_rows, int32_t& server) {
     uint64_t b = 0;

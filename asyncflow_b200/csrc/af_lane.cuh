@@ -175,7 +175,13 @@ struct Cfg {
     uint64_t* band_rows; const uint32_t* band_group; uint32_t* band_from;
     uint64_t band_first, band_n, band_group_words;
     int32_t band_groups, band_stride;
+    // per-window latency bands (run_lane<*, true> only; DESIGN.md §3.5), over the groups of band_group: window k of
+    // group g is the LAT_ROW words at lat_rows + (g * lat_windows + k) * LAT_ROW.  lat_from[local] = the completions a
+    // stopped replica added (the warp-per-replica pass adds the rest).
+    uint64_t* lat_rows; uint32_t* lat_from;
+    int32_t lat_window, lat_windows;
 };
+
 
 #if defined(__CUDACC__)
 __constant__ Cfg c_cfg;
@@ -288,7 +294,7 @@ struct St {
     uint32_t completed, flags, traced;
     uint64_t n_events;
     double lat_sum, lat_sumsq, lat_min, lat_max;
-    uint64_t* band;                             // run_lane<true>: the replica's group's difference rows
+    uint64_t* band;                             // run_lane<true, *>: the replica's group's difference rows
 };
 
 // flags that end a replica early (its partial results are written back with the flag set)
@@ -634,6 +640,35 @@ AFL_IN void band_stop(const St& W, const Mem& m) {
     AFL_C.band_from[W.local] = (uint32_t)n;
 }
 
+// ---- per-window latency bands: a completion adds one to its latency bin and its latency in 32.32 fixed point to the
+//      two sum words of its finish window, while no stop flag is set.  A flag raised during an iteration does not stop
+//      the rest of it, and what completes after the flag may differ from what the warp-per-replica engine computes;
+//      every completion before it is exact.  So the first completion after a flag records how many were added
+//      (lat_from) and ends the replica's contribution; a replica stopped without one records them all at the stop.
+//      `lat_g` is the replica's group (LAT_OFF: it adds no more), a register of run_lane's, not a member of St: the
+//      kernels without latency bands keep the exact code they had before.
+constexpr uint32_t LAT_OFF = ~0u;
+AFL_IN uint32_t lat_group(const St& W) {
+    const uint64_t i = W.replica - AFL_C.band_first;
+    return i < AFL_C.band_n ? AFL_C.band_group[i] : (uint32_t)AFL_C.band_groups;
+}
+AFL_IN void lat_add(const St& W, uint32_t& lat_g, uint32_t done, double lat) {
+    if (lat_g == LAT_OFF) return;
+    if (AFL_UNLIKELY(W.flags & STOP_FLAGS)) { AFL_C.lat_from[W.local] = done - 1u; lat_g = LAT_OFF; return; }
+    int32_t b = (int32_t)ceil(W.now) - 1;            // the throughput bucket, then its window: no division of doubles
+    b = b < 0 ? 0 : b;
+    if (b >= AFL_C.horizon_s) return;
+    const uint64_t k = (uint32_t)b / (uint32_t)AFL_C.lat_window;
+    uint64_t* row = AFL_C.lat_rows + ((uint64_t)lat_g * (uint32_t)AFL_C.lat_windows + k) * afr::LAT_ROW;
+    red_add64(row + afr::hist_bin(lat), 1u);
+    const uint64_t u = afr::lat_fixed32(lat);
+    if (u >> 32) red_add64(row + AF_HIST_BINS, u >> 32);
+    red_add64(row + AF_HIST_BINS + 1, u & 0xFFFFFFFFull);
+}
+AFL_IN void lat_stop(const St& W, uint32_t lat_g) {
+    if (lat_g != LAT_OFF) AFL_C.lat_from[W.local] = W.completed;
+}
+
 // ---- Stores (mailboxes), Containers: as af_core.cuh ----------------------------------------------------
 // is the waiter FIFO whose head is cold word `head` empty?  (n_waiting == 0: all of them are, without looking)
 AFL_IN bool q_empty(const St& W, const Mem& m, int32_t head) { return AFL_LIKELY(W.n_waiting == 0) || c32_ld(m, head) == NIL; }
@@ -724,7 +759,8 @@ static inline void red_add(uint32_t* p, uint32_t v) { *p += v; }
 #endif
 
 // client: completion (client.py:62-69 + analyzer.py:83-125)
-AFL_IN void complete(St& W, const Mem& m, uint32_t slot, double t0) {
+template <bool kLatency>
+AFL_IN void complete(St& W, const Mem& m, uint32_t slot, double t0, uint32_t& lat_g) {
     const double now = W.now;
     const double lat = now - t0;                     // finish - start (analyzer.py:86-89)
     const uint32_t done = ++W.completed;
@@ -733,11 +769,8 @@ AFL_IN void complete(St& W, const Mem& m, uint32_t slot, double t0) {
     if (lat < W.lat_min) W.lat_min = lat;
     if (lat > W.lat_max) W.lat_max = lat;
     const uint64_t local = W.local;
-    if (AFL_C.collect_hist) {
-        int32_t idx = (int32_t)(afr::d2u(lat) >> (52 - AF_HIST_SUB_BITS)) - ((1023 + AF_HIST_MIN_EXP) << AF_HIST_SUB_BITS);
-        idx = idx < 0 ? 0 : (idx >= AF_HIST_BINS ? AF_HIST_BINS - 1 : idx);
-        red_add(&AFL_C.hist[local * AF_HIST_BINS + (uint32_t)idx], 1u);
-    }
+    if (AFL_C.collect_hist) red_add(&AFL_C.hist[local * AF_HIST_BINS + (uint32_t)afr::hist_bin(lat)], 1u);
+    if constexpr (kLatency) lat_add(W, lat_g, done, lat);
     if (AFL_C.collect_thr) {                          // bucket k counts (k, k+1] (analyzer.py:108-125)
         int32_t b = (int32_t)ceil(now) - 1;
         b = b < 0 ? 0 : b;
@@ -867,13 +900,16 @@ enum : uint32_t { A_NONE = 0, A_NODE, A_STEPS, A_SEND, A_TIMER };
 // The lane's life: pull a replica, run it to the horizon, write it back, pull the next.  `next_index`
 // returns the next local replica index or ~0 when the launch has no more work for this lane.
 // `converge` is a warp-wide rendez-vous at the top of every iteration (device: __any_sync).
-// `kBands`: also accumulate the per-tick bands of the replicas' groups (Cfg.band_*); false compiles to the same code
-// as before bands existed.
+// The bands to accumulate over the replicas' groups, one flag each: `kSampled` the per-tick bands (Cfg.band_*),
+// `kLatency` the per-window latency bands (Cfg.lat_*).  <false, false> compiles to the same code as before bands
+// existed, <true, false> to the same code as before latency bands existed (two bools, not one integer mask: with an
+// integer parameter the front end emits the same kernel in a different order, and the SASS moves).
 // ---------------------------------------------------------------------------------------------------
-template <bool kBands = false, class NextFn, class ConvFn>
+template <bool kSampled = false, bool kLatency = false, class NextFn, class ConvFn>
 AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
     const Cfg& C = AFL_C;
     St W;
+    uint32_t lat_g = LAT_OFF;
     bool active = false, exhausted = false;
 #pragma unroll 1
     for (;;) {
@@ -884,7 +920,8 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
             if (r == ~0ull) exhausted = true;
             else {
                 start_replica(W, m, r);
-                if constexpr (kBands) band_start(W);
+                if constexpr (kSampled) band_start(W);
+                if constexpr (kLatency) lat_g = lat_group(W);
                 // start order of the reference (simulation_runner.py:339-342, 301-336):
                 // spike timeline, outage timeline, generator, ..., collector
                 if (C.n_spike > 0) {
@@ -974,7 +1011,8 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
         }
         AFL_SYNC();
         // ---- phase: collector ticks that fall before this event ------------------------------------------------
-        if constexpr (kBands) { if (AFL_UNLIKELY(dead)) band_stop(W, m); }     // before the frozen ticks to the horizon
+        if constexpr (kSampled) { if (AFL_UNLIKELY(dead)) band_stop(W, m); }     // before the frozen ticks to the horizon
+        if constexpr (kLatency) { if (AFL_UNLIKELY(dead)) lat_stop(W, lat_g); }
         if (run && !is_item) {
             const double tick = W.tick_time;
             if (tick < t_ev || (tick == t_ev && W.tick_seq < ev_seq)) take_ticks(W, m, t_ev, ev_seq);
@@ -997,7 +1035,7 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
         if (names_request) rq_load(W, m, slot, t0, rid, pack);
         if (is_event) {
             if (kind == K_DELIVER) {                          // edge.py:110-116: the edge's timeout fired
-                conn_add<kBands>(W, m, aux, -1);
+                conn_add<kSampled>(W, m, aux, -1);
                 const uint32_t meta = ro(C.edges + aux).meta;
                 pack += 1;                                     // record_hop(edge)
                 const uint32_t tk = (meta >> 3) & 3u;
@@ -1044,11 +1082,11 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                 consumer_get(W, m, NODE_CLIENT);
             } else if (kind == I_RAM_OK) {                     // the RAM get event is processed: the handler resumes
                 sidx = aux;
-                srv_gauge_add<kBands>(W, m, sidx, SV_RAM_IN_USE, (int32_t)ep_total_ram(m, pk_ep(pack)));
+                srv_gauge_add<kSampled>(W, m, sidx, SV_RAM_IN_USE, (int32_t)ep_total_ram(m, pk_ep(pack)));
                 act = A_STEPS;
             } else if (kind == I_CPU_OK) {                     // the CPU get event is processed
                 sidx = aux;
-                if (pack & PK_WAIT) { pack &= ~PK_WAIT; srv_gauge_add<kBands>(W, m, sidx, SV_READY_Q, -1); }
+                if (pack & PK_WAIT) { pack &= ~PK_WAIT; srv_gauge_add<kSampled>(W, m, sidx, SV_READY_Q, -1); }
                 pack |= PK_CORE;
                 act = A_STEPS;
             } else if (kind == I_CPU_PUT) {                    // waiters are re-examined, then the request goes on
@@ -1095,7 +1133,7 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                         go = false;
                     } else {
                         i32_st(m, sv_word(sidx, SV_RAM_FREE), i32_ld(m, sv_word(sidx, SV_RAM_FREE)) - (int32_t)total_ram);   // granted, and its get event would run next
-                        srv_gauge_add<kBands>(W, m, sidx, SV_RAM_IN_USE, (int32_t)total_ram);
+                        srv_gauge_add<kSampled>(W, m, sidx, SV_RAM_IN_USE, (int32_t)total_ram);
                     }
                 }
                 if (go) act = A_STEPS;
@@ -1103,7 +1141,7 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                 pack += 1;                                     // record_hop(client / LB)
                 if (node == NODE_CLIENT) {
                     if (pk_hops(pack) > 3) {                   // client.py:62: back from the servers
-                        complete(W, m, slot, t0);
+                        complete<kLatency>(W, m, slot, t0, lat_g);
                         if (can_fuse(W)) { if (from_box) consumer_get(W, m, NODE_CLIENT); }
                         else nq_push(W, m, I_CLIENT_LOOP, 0, 0);   // yield completed_box.put(state)
                     } else {
@@ -1150,7 +1188,7 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                 if (st < ep.n_steps) {
                     const StepP sp = ro(C.steps + ep.step_begin + st);
                     if (sp.kind == AF_STEP_CPU) {
-                        if (pack & PK_IO) { pack &= ~PK_IO; srv_gauge_add<kBands>(W, m, sidx, SV_IO_Q, -1); }
+                        if (pack & PK_IO) { pack &= ~PK_IO; srv_gauge_add<kSampled>(W, m, sidx, SV_IO_Q, -1); }
                         if (!(pack & PK_CORE)) {             // cpu_req = CPU.get(1); yield cpu_req
                             if (can_fuse(W) && i32_ld(m, sv_word(sidx, SV_CPU_FREE)) > 0 && q_empty(W, m, sq_word(sidx, SQ_CPUQ_HEAD))) {
                                 i32_st(m, sv_word(sidx, SV_CPU_FREE), i32_ld(m, sv_word(sidx, SV_CPU_FREE)) - 1);     // granted, and its get event would run next
@@ -1158,7 +1196,7 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                             } else {
                                 fifo_push(m, sq_word(sidx, SQ_CPUQ_HEAD), sq_word(sidx, SQ_CPUQ_TAIL), slot);
                                 W.n_waiting += 1;
-                                if (!cpu_walk(W, m, sidx, slot)) { pack |= PK_WAIT; srv_gauge_add<kBands>(W, m, sidx, SV_READY_Q, 1); }   // not cpu_req.triggered
+                                if (!cpu_walk(W, m, sidx, slot)) { pack |= PK_WAIT; srv_gauge_add<kSampled>(W, m, sidx, SV_READY_Q, 1); }   // not cpu_req.triggered
                                 break;
                             }
                         }
@@ -1173,7 +1211,7 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                             nq_push(W, m, I_CPU_PUT, sidx, slot);
                             break;
                         }
-                        if (!(pack & PK_IO)) { pack |= PK_IO; srv_gauge_add<kBands>(W, m, sidx, SV_IO_Q, 1); }
+                        if (!(pack & PK_IO)) { pack |= PK_IO; srv_gauge_add<kSampled>(W, m, sidx, SV_IO_Q, 1); }
                     }
                     const double dur = sp.c_dur >= 0 ? row_val(m, sp.c_dur) : sp.dur;
                     tm_t = W.now + dur; tm_payload = mk_payload(K_STEP_END, sidx, slot); tm_seq = W.seq++;
@@ -1191,10 +1229,10 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                     nq_push(W, m, I_CPU_PUT, sidx, slot);
                     break;
                 }
-                if (pack & PK_IO) { pack &= ~PK_IO; srv_gauge_add<kBands>(W, m, sidx, SV_IO_Q, -1); }
+                if (pack & PK_IO) { pack &= ~PK_IO; srv_gauge_add<kSampled>(W, m, sidx, SV_IO_Q, -1); }
                 const uint32_t total_ram = ep.c_ram >= 0 ? (uint32_t)row_val(m, ep.c_ram) : ep.total_ram;
                 if (total_ram) {                             // yield RAM.put(total_ram): level rises NOW
-                    srv_gauge_add<kBands>(W, m, sidx, SV_RAM_IN_USE, -(int32_t)total_ram);
+                    srv_gauge_add<kSampled>(W, m, sidx, SV_RAM_IN_USE, -(int32_t)total_ram);
                     i32_st(m, sv_word(sidx, SV_RAM_FREE), i32_ld(m, sv_word(sidx, SV_RAM_FREE)) + (int32_t)total_ram);
                     if (!can_fuse(W)) { nq_push(W, m, I_RAM_PUT, sidx, slot); break; }
                     if (AFL_UNLIKELY(!q_empty(W, m, sq_word(sidx, SQ_RAMQ_HEAD)))) ram_walk(W, m, sidx);   // the put event would run next: waiters, then forward
@@ -1290,7 +1328,7 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                     rq_release(W, m, slot);
                 } else {
                     rq_pack_set(W, m, slot, pack);              // (the one store of the record on the request's way out of a node)
-                    conn_add<kBands>(W, m, edge, 1);
+                    conn_add<kSampled>(W, m, edge, 1);
                     double effective = transit;
                     if (C.n_spike > 0) effective = transit + f64_ld(m, C.o64_spike + (int32_t)edge);   // spike read at SEND time (edge.py:94-106)
                     else effective = transit + 0.0;         // (-0.0 + 0.0 = +0.0, as with a spike table of zeros)

@@ -15,6 +15,7 @@
 #include <stdint.h>
 #include <string.h>
 #include <math.h>
+#include "../../include/asyncflow_b200.h"
 
 #if defined(__CUDACC__)
 #define AF_HD __host__ __device__ __forceinline__
@@ -87,6 +88,25 @@ AF_HD double af_div(double a, double b) {
     return __ddiv_rn(a, b);
 #else
     return a / b;
+#endif
+}
+
+// The latency histogram's bin of `lat` (AF_HIST_BINS log-linear bins, clamped at both ends): the per-replica
+// histograms and the per-window latency bands bin alike.
+AF_HD int32_t hist_bin(double lat) {
+    const int32_t idx = (int32_t)(d2u(lat) >> (52 - AF_HIST_SUB_BITS)) - ((1023 + AF_HIST_MIN_EXP) << AF_HIST_SUB_BITS);
+    return idx < 0 ? 0 : (idx >= AF_HIST_BINS ? AF_HIST_BINS - 1 : idx);
+}
+
+// A latency in 32.32 fixed point: round-to-nearest-even(lat * 2^32) (the scaling by 2^32 is exact).  Per-window latency
+// bands add these as two u64 words, so their sums are exact in whatever order the additions land.  A window of a
+// group's latency bands is LAT_ROW words: AF_HIST_BINS bin counts, the sum's high word (u >> 32), its low word.
+constexpr uint64_t LAT_ROW = AF_HIST_BINS + 2;
+AF_HD uint64_t lat_fixed32(double lat) {
+#if defined(__CUDA_ARCH__)
+    return (uint64_t)__double2ull_rn(lat * 4294967296.0);
+#else
+    return (uint64_t)nearbyint(lat * 4294967296.0);       // default rounding mode: to nearest, ties to even
 #endif
 }
 

@@ -18,6 +18,7 @@ from dataclasses import dataclass
 import numpy as np
 
 from . import _capi as K
+from .results import SweepResults, hist_percentiles
 
 N_TOTALS = 8     # completed, generated, events, replicas, overflowed, ticks, reserved x2
 
@@ -66,25 +67,7 @@ class GlobalSummary:
 
     def percentile(self, q: float) -> float:
         """numpy-'linear' percentile of ALL completions, read off the merged histogram."""
-        n = int(self.histogram.sum())
-        if n == 0:
-            return float("nan")
-        cum = np.cumsum(self.histogram)
-        base = (1023 + K.AF_HIST_MIN_EXP) << K.AF_HIST_SUB_BITS
-
-        def order_stat(rank: int) -> float:
-            b = int(np.searchsorted(cum, rank, side="right"))
-            before = int(cum[b - 1]) if b else 0
-            lo, hi = (np.array([(b + base) << (52 - K.AF_HIST_SUB_BITS),
-                                (b + 1 + base) << (52 - K.AF_HIST_SUB_BITS)], dtype=np.uint64).view(np.float64))
-            frac = ((rank - before) + 0.5) / float(self.histogram[b])
-            return float(lo + frac * (hi - lo))
-
-        pos = q / 100.0 * (n - 1)
-        lo = int(np.floor(pos))
-        frac = pos - lo
-        a = order_stat(lo)
-        return a if frac == 0.0 or lo + 1 >= n else a + frac * (order_stat(lo + 1) - a)
+        return float(hist_percentiles(self.histogram, q))
 
 
 def all_gather_summary(ints: np.ndarray, flts: np.ndarray, device: str | None = None) -> GlobalSummary:
@@ -113,6 +96,35 @@ def all_gather_summary(ints: np.ndarray, flts: np.ndarray, device: str | None = 
         replicas=int(tot[:, 3].sum()), overflowed=int(tot[:, 4].sum()),
         lat_sum=float(all_f[:, 0].sum()), lat_min=float(all_f[:, 2].min()), lat_max=float(all_f[:, 3].max()),
         per_rank_completed=[int(x) for x in tot[:, 0]])
+
+
+BAND_FIELDS = ("band_count", "band_sum", "band_sumsq", "lat_hist", "lat_sum_hi", "lat_sum_lo", "group_size")
+
+
+def all_reduce_bands(res: SweepResults, device: str | None = None) -> SweepResults:
+    """Sum the band rows of ``res`` -- the per-tick sampled-metric bands, the per-window latency bands and the group
+    sizes a rank's shard holds -- over every rank, in place, with one all-reduce: afterwards each rank holds the
+    bands of the whole sweep, as :meth:`SweepResults.concatenate` of every rank's results would.  The unsigned sums
+    travel as int64; their modular addition gives the same bits.  Works without an initialised process group."""
+    import torch  # noqa: PLC0415
+    import torch.distributed as dist  # noqa: PLC0415
+
+    present = [(k, getattr(res, k)) for k in BAND_FIELDS if getattr(res, k) is not None]
+    world = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
+    if world == 1 or not present:
+        return res
+    flat = np.concatenate([a.astype(np.uint64).view(np.int64).ravel() if a.dtype != np.int64 else a.ravel()
+                           for _, a in present])
+    dev = device or ("cuda" if dist.get_backend() == "nccl" else "cpu")
+    t = torch.from_numpy(flat).to(dev)
+    dist.all_reduce(t, op=dist.ReduceOp.SUM)
+    out = t.cpu().numpy()
+    at = 0
+    for k, a in present:
+        v = out[at:at + a.size].reshape(a.shape)
+        at += a.size
+        setattr(res, k, v.view(np.uint64).astype(a.dtype) if a.dtype != np.int64 else v.copy())
+    return res
 
 
 def run_sharded(runner, *, with_histogram: bool = True):

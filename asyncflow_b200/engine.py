@@ -33,6 +33,8 @@ class Engine:
         self._opt = K.AfOptions(0, 0, 0, 0, 1, 1, 0, 0)
         self._keep: list = []
         self._band_groups = self._run_band_groups = 0
+        self._band_opt = K.AfBandOptions(1, 0)
+        self._run_band_opt = (1, 0)
 
     # ------------------------------------------------------------------ plumbing
     def _check(self, rc: int, what: str) -> None:
@@ -91,6 +93,7 @@ class Engine:
         self._check(self._lib.af_run(self._h, int(seed), int(replica_begin), int(replica_end)), "af_run")
         self._n = int(replica_end) - int(replica_begin)
         self._run_band_groups = self._band_groups
+        self._run_band_opt = (self._band_opt.sampled, self._band_opt.latency_window_s)
 
     def sync(self) -> None:
         self._check(self._lib.af_sync(self._h), "af_sync")
@@ -172,6 +175,29 @@ class Engine:
         self._check(self._lib.af_bands_upload(self._h, g.ctypes.data, g.size, int(first_replica), n_groups),
                     "af_bands_upload")
         self._band_groups = n_groups
+
+    def configure_bands(self, *, sampled: bool = True, latency_window_s: int = 0) -> None:
+        """Which bands the uploaded groups accumulate from the next run on: the per-tick sampled-metric bands
+        (:meth:`bands`) and / or per-window latency bands of ``latency_window_s`` whole seconds (0: off;
+        :meth:`latency_bands`) -- ``af_bands_configure``."""
+        opt = K.AfBandOptions(int(bool(sampled)), int(latency_window_s))
+        self._check(self._lib.af_bands_configure(self._h, C.byref(opt)), "af_bands_configure")
+        self._band_opt = opt
+
+    def latency_bands(self) -> tuple[np.ndarray, np.ndarray, np.ndarray]:
+        """Latency bands of the last run: ``(hist [G, W, AF_HIST_BINS] u64, sum_hi [G, W] u64, sum_lo [G, W] u64)`` --
+        per group and window, the completions per latency bin and the two words of their latencies' 32.32 fixed-point
+        sum, ``sum_hi * 2**32 + sum_lo`` (``af_fetch_latency_bands``)."""
+        G, w = self._run_band_groups, self._run_band_opt[1]
+        cap = -(-int(self.flat.horizon_s) // max(int(w), 1))
+        hist = np.empty((G, cap, K.AF_HIST_BINS), dtype=np.uint64)
+        hi = np.empty((G, cap), dtype=np.uint64)
+        lo = np.empty((G, cap), dtype=np.uint64)
+        n = C.c_uint64()
+        self._check(self._lib.af_fetch_latency_bands(self._h, hist.ctypes.data, hi.ctypes.data, lo.ctypes.data, cap,
+                                                     C.byref(n)), "af_fetch_latency_bands")
+        W = n.value
+        return hist[:, :W], hi[:, :W], lo[:, :W]
 
     def bands(self) -> tuple[np.ndarray, np.ndarray, np.ndarray]:
         """Bands of the last run: ``(count [G, T] u32, sum [G, S, T] u64, sumsq [G, S, T] u64)`` -- per group, series

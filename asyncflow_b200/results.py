@@ -34,6 +34,52 @@ EDGE_SERIES = "edge_concurrent_connection"
 LATENCY_ORDER = ("total_requests", "mean", "median", "std_dev", "p95", "p99", "min", "max")
 
 
+def hist_percentiles(hist: np.ndarray, q: float) -> np.ndarray:
+    """numpy-'linear' percentile ``q`` of the completions each latency histogram counts (``hist[..., AF_HIST_BINS]``,
+    the log-linear bins of the engine): the two order statistics around ``q / 100 * (n - 1)``, each placed inside its
+    bin by its rank among the bin's counts, interpolated linearly.  NaN where a histogram is empty.  Returns
+    ``hist.shape[:-1]``."""
+    h = np.asarray(hist)
+    flat = h.reshape(-1, h.shape[-1])
+    out = np.full(flat.shape[0], np.nan)
+    base = (1023 + K.AF_HIST_MIN_EXP) << K.AF_HIST_SUB_BITS
+    for c in range(0, flat.shape[0], 1024):                   # bounded temporaries: [rows, bins] at a time
+        cum = np.cumsum(flat[c:c + 1024], axis=1, dtype=np.int64)
+        n = cum[:, -1]
+        ok = n > 0
+        if not ok.any():
+            continue
+        cum, n = cum[ok], n[ok]
+        rows = flat[c:c + 1024][ok]
+
+        def order_stat(rank: np.ndarray, cum=cum, rows=rows) -> np.ndarray:
+            b = (cum <= rank[:, None]).sum(axis=1)          # searchsorted(cum, rank, side="right") per row
+            b = np.minimum(b, cum.shape[1] - 1)
+            before = np.where(b > 0, cum[np.arange(b.size), np.maximum(b - 1, 0)], 0)
+            lo = ((b + base).astype(np.uint64) << np.uint64(52 - K.AF_HIST_SUB_BITS)).view(np.float64)
+            hi = ((b + 1 + base).astype(np.uint64) << np.uint64(52 - K.AF_HIST_SUB_BITS)).view(np.float64)
+            frac = ((rank - before).astype(np.float64) + 0.5) / rows[np.arange(b.size), b].astype(np.float64)
+            return lo + frac * (hi - lo)
+
+        pos = q / 100.0 * (n - 1).astype(np.float64)
+        lo = np.floor(pos)
+        frac = pos - lo
+        lo = lo.astype(np.int64)
+        a = order_stat(lo)
+        nxt = np.minimum(lo + 1, n - 1)
+        b = order_stat(nxt)
+        out[c + np.flatnonzero(ok)] = np.where((frac == 0.0) | (lo + 1 >= n), a, a + frac * (b - a))
+    return out.reshape(h.shape[:-1])
+
+
+def fixed32_mean(sum_hi: np.ndarray, sum_lo: np.ndarray, n: np.ndarray) -> np.ndarray:
+    """Mean latency from the two words of a 32.32 fixed-point latency sum (``sum_hi * 2**32 + sum_lo``) over ``n``
+    completions; NaN where ``n == 0``."""
+    s = np.asarray(sum_hi).astype(np.float64) + np.asarray(sum_lo).astype(np.float64) * 2.0 ** -32
+    with np.errstate(invalid="ignore", divide="ignore"):
+        return np.where(n > 0, s / np.maximum(n, 1), np.nan)
+
+
 class _Name(str):
     """A metric name that also answers ``.value`` like the reference's StrEnum."""
 
@@ -187,6 +233,14 @@ class SweepResults:
         self.band_count: np.ndarray | None = None
         self.band_sum: np.ndarray | None = None
         self.band_sumsq: np.ndarray | None = None
+        # per-window latency bands (SweepRunner(latency_window_s=w)): per group g and window k of w seconds, the
+        # completions per latency bin [G, W, AF_HIST_BINS] u64 and the two words of their latencies' 32.32 fixed-point
+        # sum [G, W] u64; the replicas of each group [G]
+        self.lat_window_s: int = 0
+        self.lat_hist: np.ndarray | None = None
+        self.lat_sum_hi: np.ndarray | None = None
+        self.lat_sum_lo: np.ndarray | None = None
+        self.group_size: np.ndarray | None = None
 
     def __len__(self) -> int:
         return int(self.stats.shape[0])
@@ -280,6 +334,9 @@ class SweepResults:
                            self.replica_begin)
         out.traced = self.traced
         out.band_count, out.band_sum, out.band_sumsq = self.band_count, self.band_sum, self.band_sumsq
+        out.lat_window_s, out.lat_hist, out.lat_sum_hi, out.lat_sum_lo = (self.lat_window_s, self.lat_hist,
+                                                                          self.lat_sum_hi, self.lat_sum_lo)
+        out.group_size = self.group_size
         return out
 
     def bands(self, key: Any, entity_id: str) -> dict[str, np.ndarray]:
@@ -328,6 +385,37 @@ class SweepResults:
         return {"t": np.arange(T) * self.flat.sample_period, "n": self.band_count, "mean": mean, "std": std,
                 "lo": mean - half, "hi": mean + half}
 
+    def group_latency(self) -> dict[str, Any]:
+        """Per group and window, over the group's replicas, the latency and throughput of the completions that
+        finish in the window (``SweepRunner(latency_window_s=w)``): ``{"t", "n", "rps", "mean", "p50", "p95",
+        "p99", "total"}``.  ``t`` (``[W]``, seconds) are the window ends, the ``ts`` of ``get_throughput_series(w)``
+        (``metrics/analyzer.py:187-216``; a last window cut at the horizon ends there); the rest are ``[G, W]``:
+        ``n`` completions, ``rps`` = n / (window width x replicas in the group), comparable with one replica's
+        throughput series, the mean from the exact fixed-point sums, and histogram percentiles as in
+        :attr:`stats`.  ``total`` holds the same statistics (``[G]``) over the whole run, as
+        ``get_latency_stats`` (``analyzer.py:83-105``) lifted to a group.  NaN where a window has no completion."""
+        if self.lat_hist is None:
+            msg = "no latency bands: run the sweep with SweepRunner(bands=..., latency_window_s=w)"
+            raise ValueError(msg)
+        w, H = int(self.lat_window_s), int(self.flat.horizon_s)
+        G, W = self.lat_sum_hi.shape
+        start = np.arange(W, dtype=np.float64) * w
+        end = np.minimum(start + w, float(H))
+        size = np.asarray(self.group_size, dtype=np.float64)
+
+        def stats(hist, hi, lo, width):
+            n = hist.sum(axis=-1, dtype=np.uint64)
+            with np.errstate(invalid="ignore", divide="ignore"):
+                rps = n.astype(np.float64) / (width * size.reshape(size.shape + (1,) * (n.ndim - 1)))
+            return {"n": n, "rps": rps, "mean": fixed32_mean(hi, lo, n), "p50": hist_percentiles(hist, 50.0),
+                    "p95": hist_percentiles(hist, 95.0), "p99": hist_percentiles(hist, 99.0)}
+
+        out: dict[str, Any] = {"t": end}
+        out.update(stats(self.lat_hist, self.lat_sum_hi, self.lat_sum_lo, (end - start)[None, :]))
+        out["total"] = stats(self.lat_hist.sum(axis=1, dtype=np.uint64), self.lat_sum_hi.sum(axis=1, dtype=np.uint64),
+                             self.lat_sum_lo.sum(axis=1, dtype=np.uint64), float(H))
+        return out
+
     @staticmethod
     def concatenate(parts: list["SweepResults"]) -> "SweepResults":
         f = parts[0]
@@ -341,4 +429,11 @@ class SweepResults:
             out.band_count = np.sum([p.band_count for p in parts], axis=0, dtype=np.uint32)
             out.band_sum = np.sum([p.band_sum for p in parts], axis=0, dtype=np.uint64)
             out.band_sumsq = np.sum([p.band_sumsq for p in parts], axis=0, dtype=np.uint64)
+        if all(p.lat_hist is not None for p in parts):
+            out.lat_window_s = f.lat_window_s
+            out.lat_hist = np.sum([p.lat_hist for p in parts], axis=0, dtype=np.uint64)
+            out.lat_sum_hi = np.sum([p.lat_sum_hi for p in parts], axis=0, dtype=np.uint64)
+            out.lat_sum_lo = np.sum([p.lat_sum_lo for p in parts], axis=0, dtype=np.uint64)
+        if all(p.group_size is not None for p in parts):
+            out.group_size = np.sum([p.group_size for p in parts], axis=0, dtype=np.int64)
         return out

@@ -38,7 +38,7 @@
 extern "C" {
 #endif
 
-#define AF_ABI_VERSION 3
+#define AF_ABI_VERSION 4
 
 typedef enum AfStatus {
     AF_OK = 0,
@@ -277,6 +277,28 @@ int af_bands_upload(af_engine* e, const uint32_t* group_of, uint64_t n, uint64_t
  * capacity_ticks entries; *n_ticks = the run's tick count.  Any of the three arrays may be NULL (not fetched). */
 int af_fetch_bands(af_engine* e, uint32_t* count, uint64_t* sum, uint64_t* sumsq,
                    uint64_t capacity_ticks, uint64_t* n_ticks);
+
+/* Which bands af_run accumulates over the groups of af_bands_upload (defaults: {1, 0}, the per-tick bands alone).
+ * latency_window_s = w > 0 adds per-window latency bands: window k < n_windows = ceil(horizon_s / w) holds the
+ * completions whose finish time lies in (k w, min((k + 1) w, horizon)] (k = (ceil(finish) - 1) / w in integers, as the
+ * throughput buckets), and per group g and window k the device accumulates
+ *   hist[g][k][AF_HIST_BINS]   completions per latency bin (the bins of the per-replica histograms)
+ *   sum_hi[g][k], sum_lo[g][k] the sum of u = round-to-nearest(latency x 2^32) as sum(u >> 32) and sum(u & 0xFFFFFFFF):
+ *                              hi x 2^32 + lo is the exact fixed-point sum while a window has < 2^32 completions
+ * A completion counts while its replica has no stop flag; a replica the thread-per-replica pass flags and the
+ * warp-per-replica pass re-runs inside the same af_run counts once, in full; host-side re-runs add nothing.  Every
+ * other output is the same with latency bands on or off.  Rejected (AF_ERR_INVALID) when w < 0, or when the rows,
+ * (n_groups + 1) x n_windows x (AF_HIST_BINS + 2) x 8 bytes, exceed the device's memory; af_bands_upload and af_run
+ * check the rows again. */
+typedef struct AfBandOptions {
+    int32_t sampled;            /* per-tick sampled-metric bands (af_fetch_bands): 1 by default      */
+    int32_t latency_window_s;   /* 0: off (default); else per-window latency bands of this width (s)  */
+} AfBandOptions;
+int af_bands_configure(af_engine* e, const AfBandOptions* opt);
+/* latency bands of the last af_run: hist[g][k][AF_HIST_BINS], sum_hi[g][k], sum_lo[g][k] for k < min(*n_windows,
+ * capacity_windows), capacity_windows windows per group; *n_windows = the run's window count.  Any array may be NULL. */
+int af_fetch_latency_bands(af_engine* e, uint64_t* hist, uint64_t* sum_hi, uint64_t* sum_lo,
+                           uint64_t capacity_windows, uint64_t* n_windows);
 
 /* AF-RNG known-answer hook: the device's random numbers outside the state machine, n values per call
  * (the streams of oracle/afrng.py; tests/test_gpu_rng.py compares them bit for bit with oracle/afrng_c):
