@@ -89,11 +89,13 @@ __global__ void AF_LAUNCH_BOUNDS af_sim_kernel(const afc::BandArgs band) {
 // lane decides the CTA size at launch).  More warps shrink each lane's share of shared memory (more of the heap lives
 // in L2), so the register budget is spent at 12 warps: 158 registers on sm_90a, no spills.  kSampled / kLatency: the
 // same kernel also accumulating the per-tick / per-window latency bands of the uploaded groups (af_run picks the one
-// the band options ask for); <false, false> is the kernel without them.
+// the band options ask for); <false, false> is the kernel without them.  kLean: the loop without spikes, outages,
+// traces, the general edge sampler and the endpoint draw (af_run picks it when aflh::lean_launch says the launch can
+// reach none of them).
 #ifndef AF_LANE_MAX_THREADS
 #define AF_LANE_MAX_THREADS 384
 #endif
-template <bool kSampled = false, bool kLatency = false>
+template <bool kSampled = false, bool kLatency = false, bool kLean = false>
 __global__ void __launch_bounds__(AF_LANE_MAX_THREADS, 1) af_lane_kernel() {
     const afl::Cfg& C = afl::c_cfg;
     const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
@@ -106,7 +108,7 @@ __global__ void __launch_bounds__(AF_LANE_MAX_THREADS, 1) af_lane_kernel() {
     m.g128 = gs + lane * 16u;
     m.g64 = gs + (size_t)C.gn128 * afl::STRIDE128 + lane * 8u;
     m.g32 = gs + (size_t)C.gn128 * afl::STRIDE128 + (size_t)C.gn64 * afl::STRIDE64 + lane * 4u;
-    afl::run_lane<kSampled, kLatency>(m,
+    afl::run_lane<kSampled, kLatency, kLean>(m,
         [&]() -> uint64_t {
             const unsigned long long k = atomicAdd(C.work_counter, 1ull);
             return k < C.n_replicas ? (uint64_t)C.order[k] : ~0ull;
@@ -360,7 +362,7 @@ struct af_engine {
     DevBuf d_l_edges, d_l_servers, d_l_eps, d_l_steps, d_l_spikes, d_l_outages, d_l_lb, d_l_cols, d_gtier, d_redo_list, d_redo_count, d_counter2;
     afl::Cfg C_host{};
     int32_t last_ev_s = 0, last_rq_s = 0;          // the pool split of the launch's heaviest replica (AfRunPasses)
-    bool last_lane = false, last_warp = false; int last_lane_warps = 0;
+    bool last_lane = false, last_warp = false, last_lean = false; int last_lane_warps = 0;
     // spill + outputs
     DevBuf d_sp_evt, d_sp_evk, d_sp_rq, d_sp_nx;
     DevBuf d_okey, d_oidx, d_order, d_okey64, d_sort_tmp;     // pull order (af_order_*_kernel + radix sorts)
@@ -796,8 +798,13 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
     }
     // thread-per-replica: one persistent CTA per SM
     uint64_t lgrid = 0; size_t lsmem = 0;
-    void (*lane_kernel)() = bands ? (lat ? af_lane_kernel<true, true> : af_lane_kernel<true, false>)
-                                  : (lat ? af_lane_kernel<false, true> : af_lane_kernel<false, false>);
+    // the lean build of the loop when the launch cannot reach what it leaves out; ASYNCFLOW_B200_LANE_FULL (A/B
+    // experiments) keeps the full one
+    const bool lean = lane && aflh::lean_launch(e->sc, o.trace_replicas) && getenv("ASYNCFLOW_B200_LANE_FULL") == nullptr;
+    void (*lane_kernel)() = lean ? (bands ? (lat ? af_lane_kernel<true, true, true> : af_lane_kernel<true, false, true>)
+                                          : (lat ? af_lane_kernel<false, true, true> : af_lane_kernel<false, false, true>))
+                                 : (bands ? (lat ? af_lane_kernel<true, true> : af_lane_kernel<true, false>)
+                                          : (lat ? af_lane_kernel<false, true> : af_lane_kernel<false, false>));
     if (lane) {
         lsmem = (size_t)lane_warps * (size_t)C.warp_bytes;
         AF_CUDA(e, cudaFuncSetAttribute(lane_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lsmem), "smem attribute");
@@ -992,7 +999,7 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
     }
     AF_CUDA(e, cudaEventRecord(e->ev_end, e->stream), "event");
     e->last_n = n; e->ran = true; e->timing_valid = false;
-    e->last_lane = lane; e->last_warp = warp; e->last_lane_warps = lane_warps;
+    e->last_lane = lane; e->last_warp = warp; e->last_lean = lean; e->last_lane_warps = lane_warps;
     e->last_bands = bands; e->last_band_groups = e->band_groups; e->last_band_ticks = (uint32_t)band_ticks;
     e->last_band_stride = band_stride;
     e->last_lat = lat; e->last_lat_groups = e->band_groups; e->last_lat_windows = lat_windows;
@@ -1036,6 +1043,7 @@ int af_last_run_passes(af_engine* e, AfRunPasses* out) {
     out->lane_bytes = e->last_lane ? e->C_host.warp_bytes / 32 : 0;
     out->lane_events_smem = e->last_lane ? e->last_ev_s : 0; out->lane_requests_smem = e->last_lane ? e->last_rq_s : 0;
     out->lane_pool_elems = e->last_lane ? e->C_host.pool : 0;
+    out->lane_lean = e->last_lean ? 1 : 0;
     out->lane_replicas = e->last_lane ? e->last_n : 0;
     out->warp_replicas = e->last_warp ? e->last_n : 0;
     if (e->last_lane && e->last_warp) {

@@ -593,13 +593,14 @@ AFL_IN bool gauge_on(int32_t j) {
                                    : (AFL_C.metrics_mask & AF_METRIC_EDGE_CONN) != 0;
 }
 // every collector tick ordered before (t, ev_seq)
+template <bool kLean>
 AFL_IN void take_ticks(St& W, const Mem& m, double t, uint32_t ev_seq) {
     double tick = W.tick_time;
     uint32_t tseq = W.tick_seq, nt = W.n_ticks, seq = W.seq;
     const double horizon = W.horizon;
 #pragma unroll 1
     while ((tick < t || (tick == t && tseq < ev_seq)) && tick < horizon) {
-        if (AFL_UNLIKELY(W.traced != 0) && (int32_t)nt < AFL_C.trace_tick_cap) {
+        if (!kLean && AFL_UNLIKELY(W.traced != 0) && (int32_t)nt < AFL_C.trace_tick_cap) {
 #pragma unroll 1
             for (int32_t j = 0; j < AFL_C.n_series; ++j)
                 if (gauge_on(j)) AFL_C.trace_series[(W.local * (uint64_t)AFL_C.n_series + (uint32_t)j) * (uint64_t)AFL_C.trace_tick_cap + nt] = gauge_value(m, j);
@@ -759,7 +760,7 @@ static inline void red_add(uint32_t* p, uint32_t v) { *p += v; }
 #endif
 
 // client: completion (client.py:62-69 + analyzer.py:83-125)
-template <bool kLatency>
+template <bool kLatency, bool kLean>
 AFL_IN void complete(St& W, const Mem& m, uint32_t slot, double t0, uint32_t& lat_g) {
     const double now = W.now;
     const double lat = now - t0;                     // finish - start (analyzer.py:86-89)
@@ -776,16 +777,20 @@ AFL_IN void complete(St& W, const Mem& m, uint32_t slot, double t0, uint32_t& la
         b = b < 0 ? 0 : b;
         if (b < AFL_C.horizon_s) red_add(&AFL_C.thr[local * (uint64_t)AFL_C.horizon_s + (uint32_t)b], 1u);
     }
-    if (AFL_UNLIKELY(W.traced != 0)) {
-        if ((int32_t)(done - 1) < AFL_C.trace_clock_cap) {
-            double* p = AFL_C.trace_clocks + (local * (uint64_t)AFL_C.trace_clock_cap + (done - 1)) * 2;
-            p[0] = t0; p[1] = now;
-        } else W.flags |= AF_FLAG_TRACE_TRUNCATED;
+    if constexpr (!kLean) {              // (`if (!kLean && ...)` here moves the SASS of the full kernel)
+        if (AFL_UNLIKELY(W.traced != 0)) {
+            if ((int32_t)(done - 1) < AFL_C.trace_clock_cap) {
+                double* p = AFL_C.trace_clocks + (local * (uint64_t)AFL_C.trace_clock_cap + (done - 1)) * 2;
+                p[0] = t0; p[1] = now;
+            } else W.flags |= AF_FLAG_TRACE_TRUNCATED;
+        }
     }
     rq_release(W, m, slot);
 }
 
 // ---- set-up / write-back (once per replica) -----------------------------------------------------------------
+// (kLean: see run_lane -- no spike offsets, no traced replica)
+template <bool kLean>
 AFL_IN void start_replica(St& W, const Mem& m, uint64_t local_index) {
     const Cfg& C = AFL_C;
     W.local = local_index;
@@ -806,12 +811,12 @@ AFL_IN void start_replica(St& W, const Mem& m, uint64_t local_index) {
     W.lb_n = C.n_lb_edges; W.spike_cur = 0; W.outage_cur = 0;
     W.n_ticks = 0; W.completed = 0; W.flags = 0; W.n_events = 0;
     W.lat_sum = 0.0; W.lat_sumsq = 0.0; W.lat_min = afr::u2d(INF_BITS); W.lat_max = 0.0;
-    W.traced = (int64_t)local_index < (int64_t)C.trace_replicas ? 1u : 0u;
+    if constexpr (!kLean) W.traced = (int64_t)local_index < (int64_t)C.trace_replicas ? 1u : 0u;
     W.users_mean = C.users_mean; W.users_sigma = C.users_sigma; W.rate_per_user = C.rate_per_user;
 #pragma unroll 1
     for (int32_t i = 0; i < C.n_edges; ++i) {
         w32_st(m, C.o32_conn + i, 0); *g32p(m, C.gi_sent + i) = 0; c32_st(m, C.c_drop + i, 0);
-        if (C.n_spike > 0) f64_st(m, C.o64_spike + i, 0.0);
+        if (!kLean && C.n_spike > 0) f64_st(m, C.o64_spike + i, 0.0);
     }
 #pragma unroll 1
     for (int32_t i = 0; i < C.n_servers; ++i) {
@@ -853,6 +858,7 @@ AFL_IN void start_replica(St& W, const Mem& m, uint64_t local_index) {
     }
 }
 
+template <bool kLean>
 AFL_IN void write_back(St& W, const Mem& m) {
     const Cfg& C = AFL_C;
     const uint64_t local = W.local;
@@ -880,7 +886,7 @@ AFL_IN void write_back(St& W, const Mem& m) {
     st.lat_min = W.completed ? W.lat_min : 0.0; st.lat_max = W.lat_max;
     st.p50 = st.p95 = st.p99 = afr::u2d(0x7FF8000000000000ull);
     C.stats[local] = st;
-    if (W.traced) { C.trace_counts[local * 2] = W.completed; C.trace_counts[local * 2 + 1] = W.n_ticks; }
+    if (!kLean && W.traced) { C.trace_counts[local * 2] = W.completed; C.trace_counts[local * 2 + 1] = W.n_ticks; }
 }
 
 // what a phase hands to the next one
@@ -904,8 +910,11 @@ enum : uint32_t { A_NONE = 0, A_NODE, A_STEPS, A_SEND, A_TIMER };
 // `kLatency` the per-window latency bands (Cfg.lat_*).  <false, false> compiles to the same code as before bands
 // existed, <true, false> to the same code as before latency bands existed (two bools, not one integer mask: with an
 // integer parameter the front end emits the same kernel in a different order, and the SASS moves).
+// `kLean`: the launch has no spikes, no outages, no traced replica, only normal and exponential edges and one endpoint
+// per server (aflh::lean_launch); the code for those features is left out of the loop, which does the same work in
+// the same order with fewer instructions to fetch.  <S, L, false> compiles to the same code as before kLean existed.
 // ---------------------------------------------------------------------------------------------------
-template <bool kSampled = false, bool kLatency = false, class NextFn, class ConvFn>
+template <bool kSampled = false, bool kLatency = false, bool kLean = false, class NextFn, class ConvFn>
 AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
     const Cfg& C = AFL_C;
     St W;
@@ -919,18 +928,18 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
             const uint64_t r = next_index();
             if (r == ~0ull) exhausted = true;
             else {
-                start_replica(W, m, r);
+                start_replica<kLean>(W, m, r);
                 if constexpr (kSampled) band_start(W);
                 if constexpr (kLatency) lat_g = lat_group(W);
                 // start order of the reference (simulation_runner.py:339-342, 301-336):
                 // spike timeline, outage timeline, generator, ..., collector
-                if (C.n_spike > 0) {
+                if (!kLean && C.n_spike > 0) {
                     double f = ro(C.spikes).fire;
                     bool arm = true;
                     if (f == 0.0) arm = on_spike(W, m, f);
                     if (arm && f < W.horizon) { if (f == W.now) W.busy |= 1u; heap_push(W, m, afr::d2u(f), ((uint64_t)(W.seq++) << 32) | mk_payload(K_SPIKE, 0, 0)); }
                 }
-                if (C.n_outage > 0) {
+                if (!kLean && C.n_outage > 0) {
                     double f = ro(C.outages).fire;
                     bool arm = true;
                     if (f == 0.0) arm = on_outage(W, m, f);
@@ -1015,9 +1024,9 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
         if constexpr (kLatency) { if (AFL_UNLIKELY(dead)) lat_stop(W, lat_g); }
         if (run && !is_item) {
             const double tick = W.tick_time;
-            if (tick < t_ev || (tick == t_ev && W.tick_seq < ev_seq)) take_ticks(W, m, t_ev, ev_seq);
+            if (tick < t_ev || (tick == t_ev && W.tick_seq < ev_seq)) take_ticks<kLean>(W, m, t_ev, ev_seq);
         }
-        if (AFL_UNLIKELY(finish)) { write_back(W, m); active = false; }
+        if (AFL_UNLIKELY(finish)) { write_back<kLean>(W, m); active = false; }
         AFL_SYNC();
         if (is_event) { W.now = t_ev; W.n_events += 1; }
 
@@ -1050,7 +1059,7 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                 sidx = aux;
                 pack += (1u << 8);                             // the timeout fired: next step
                 act = A_STEPS;
-            } else if (kind == K_ARRIVAL) {                   // rqs_generator.py:97-119
+            } else if (kLean || kind == K_ARRIVAL) {          // rqs_generator.py:97-119 (lean: the only kind left)
                 rid = ++W.generated;
                 slot = rq_alloc(W, m);
                 // the generator asks the sampler for the next gap right after transport(): its timeout is
@@ -1113,7 +1122,7 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                 const ServerP sp = ro(C.servers + sidx);
                 pack += 1;                                     // record_hop(SERVER)
                 uint32_t epi = 0;
-                if (sp.n_ep > 1) {
+                if (!kLean && sp.n_ep > 1) {
                     afr::Src src = afr::make_request(C.seed, W.replica, afr::P_SERVER, rid, pk_hops(pack));
                     src.load(0);
                     epi = (uint32_t)(((uint64_t)src.w.x * sp.n_ep) >> 32);
@@ -1141,7 +1150,7 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                 pack += 1;                                     // record_hop(client / LB)
                 if (node == NODE_CLIENT) {
                     if (pk_hops(pack) > 3) {                   // client.py:62: back from the servers
-                        complete<kLatency>(W, m, slot, t0, lat_g);
+                        complete<kLatency, kLean>(W, m, slot, t0, lat_g);
                         if (can_fuse(W)) { if (from_box) consumer_get(W, m, NODE_CLIENT); }
                         else nq_push(W, m, I_CLIENT_LOOP, 0, 0);   // yield completed_box.put(state)
                     } else {
@@ -1264,11 +1273,11 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                 sigma = E.c_sigma >= 0 ? row_val(m, E.c_sigma) : E.sigma;
                 dist = (int)(E.meta & 7u);
             }
-            const bool fast = send && (dist == 1 /*NORMAL*/ || dist == 3 /*EXPONENTIAL*/);
+            const bool fast = kLean ? send : send && (dist == 1 /*NORMAL*/ || dist == 3 /*EXPONENTIAL*/);
             const bool ride = !send && (is_event || is_item) && !finish && W.gap_cnt < 2u && !W.g_done
                               && W.g_vnow < W.horizon && W.g_vnow < W.g_wend && W.g_lam > 0.0;
             double u = 0.0, transit = 0.0;
-            if (send && !fast) {                             // the other distributions: the general sampler, out of line
+            if (!kLean && send && !fast) {                   // the other distributions: the general sampler, out of line
                 const afr::EdgeDraw d = afr::edge_draw(C.seed, W.replica, rid, pk_hops(pack), dist, mean, sigma, dropout);
                 u = d.u; transit = d.transit;
             }
@@ -1330,7 +1339,7 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                     rq_pack_set(W, m, slot, pack);              // (the one store of the record on the request's way out of a node)
                     conn_add<kSampled>(W, m, edge, 1);
                     double effective = transit;
-                    if (C.n_spike > 0) effective = transit + f64_ld(m, C.o64_spike + (int32_t)edge);   // spike read at SEND time (edge.py:94-106)
+                    if (!kLean && C.n_spike > 0) effective = transit + f64_ld(m, C.o64_spike + (int32_t)edge);   // spike read at SEND time (edge.py:94-106)
                     else effective = transit + 0.0;         // (-0.0 + 0.0 = +0.0, as with a spike table of zeros)
                     tm_t = W.now + effective; tm_payload = mk_payload(K_DELIVER, edge, slot); tm_seq = s;
                     act = A_TIMER;

@@ -192,6 +192,17 @@ inline void pool_split(const afl::Cfg& C, int32_t need, int32_t& ev_s, int32_t& 
     rq_s = C.pool - ev_s;
 }
 
+// Does a launch qualify for the lean lane kernel (run_lane<*, *, true>)?  No spikes, no outages, no traced replica,
+// every edge normal or exponential, every server with one endpoint.  No sweep column can change any of these.
+inline bool lean_launch(const AfScenario& s, int32_t trace_replicas) {
+    if (s.n_spike_marks > 0 || s.n_outage_marks > 0 || trace_replicas > 0) return false;
+    for (int i = 0; i < s.n_edges; ++i)
+        if (s.edges[i].dist != AF_DIST_NORMAL && s.edges[i].dist != AF_DIST_EXPONENTIAL) return false;
+    for (int i = 0; i < s.n_servers; ++i)
+        if (s.servers[i].n_endpoints != 1) return false;
+    return true;
+}
+
 // `ev_need`: pending-events estimate of the replicas the launch has no per-replica estimate for (Cfg.row_need; 0: the
 // even split -- the twin's default); `rq_min`: the record slots that stay in shared memory when the events take more
 // than the even split.

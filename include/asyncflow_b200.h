@@ -38,7 +38,7 @@
 extern "C" {
 #endif
 
-#define AF_ABI_VERSION 4
+#define AF_ABI_VERSION 5
 
 typedef enum AfStatus {
     AF_OK = 0,
@@ -238,6 +238,8 @@ typedef struct AfRunPasses {
     uint64_t lane_replicas;              /* replicas the thread-per-replica pass ran                     */
     uint64_t warp_replicas;              /* replicas the warp-per-replica pass ran (AUTO: the flagged)   */
     int32_t lane_pool_elems;             /* 16-byte elements of a lane's pool (heap entries + records)   */
+    int32_t lane_lean;                   /* 1: the lane pass ran the lean build of its loop (no spikes,
+                                            outages, traces, general edge samplers or endpoint draws)    */
 } AfRunPasses;
 int af_last_run_passes(af_engine* e, AfRunPasses* out);
 
