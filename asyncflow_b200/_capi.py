@@ -11,7 +11,7 @@ from __future__ import annotations
 import ctypes as C
 from pathlib import Path
 
-AF_ABI_VERSION = 5
+AF_ABI_VERSION = 6
 AF_HIST_BINS = 4096
 AF_HIST_SUB_BITS = 7
 AF_HIST_MIN_EXP = -20
@@ -138,6 +138,7 @@ EXPORTS = [
     "af_fetch_histograms", "af_fetch_throughput", "af_fetch_sampled", "af_fetch_trace_clocks",
     "af_fetch_trace_series", "af_reduce_histograms", "af_engine_set_mode", "af_last_run_passes",
     "af_selftest_rng", "af_bands_upload", "af_fetch_bands", "af_bands_configure", "af_fetch_latency_bands",
+    "af_dist_bands_configure", "af_fetch_dist_bands",
 ]
 
 _lib = None
@@ -185,6 +186,8 @@ def load() -> C.CDLL:
     lib.af_fetch_bands.argtypes = [vp, vp, vp, vp, u64, C.POINTER(u64)]
     lib.af_bands_configure.argtypes = [vp, C.POINTER(AfBandOptions)]
     lib.af_fetch_latency_bands.argtypes = [vp, vp, vp, vp, u64, C.POINTER(u64)]
+    lib.af_dist_bands_configure.argtypes = [vp, vp, C.c_int32]
+    lib.af_fetch_dist_bands.argtypes = [vp, vp, u64, C.POINTER(u64), C.POINTER(C.c_uint32)]
     for name in EXPORTS:
         fn = getattr(lib, name)
         if fn.restype is C.c_int and name not in ("af_abi_version",):

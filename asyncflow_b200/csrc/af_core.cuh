@@ -180,6 +180,11 @@ struct State {
     // pass already added (a re-run adds from there on), the window width in seconds
     uint64_t* lat;
     uint32_t lat_from, lat_window;
+    // per-tick distribution bands: the replica's group's rows (nullptr: off; the first tick is band_from, the last
+    // emitted values are the band_prev table), each series' slot (-1: not selected), bins per tick row, words per series
+    uint32_t* dist; const int32_t* dist_slot;
+    uint64_t dist_series_words;
+    uint32_t dist_bins, dist_pad;
 };
 
 // Everything the kernel needs to know about sizes; built on the host.
@@ -213,6 +218,11 @@ struct BandArgs {
     uint32_t groups, stride; int32_t prev_off, pad;
     uint64_t* lat_rows; const uint32_t* lat_from;
     uint32_t lat_window, lat_windows;
+    // per-tick distribution bands (dist_rows == nullptr: off), over the same groups and with the same from[] as the
+    // per-tick bands: afl::Cfg's dist_* (af_lane.cuh); they need the prev_off table too
+    uint32_t* dist_rows; const int32_t* dist_slot;
+    uint64_t dist_group_words, dist_series_words;
+    uint32_t dist_bins, dist_pad;
 };
 
 constexpr int32_t NQ_CAP = 128;   // now-queue capacity (power of two)
@@ -950,8 +960,13 @@ AF_FN void take_samples(State& W, double t, uint32_t ev_seq) {
     // per-tick bands: from tick band_from on, a series whose value differs from the last one emitted adds the difference
     // (and that of the squares) at this tick's index of the group's difference rows -- the lane engine's contract,
     // evaluated at the ticks instead of at the changes; the first tick emits the full value and joins the count
+    // Distribution bands likewise: from band_from on, a selected series whose value differs from the last one emitted
+    // moves from bin(prev) to bin(v) at this tick (nothing when the bin stays); the first tick adds bin(v) alone.  Both
+    // kinds read the last emitted value before it is updated.
     uint64_t* const band = W.band;
     const uint64_t stride = W.band_stride, sq = (uint64_t)n_series * stride;
+    uint32_t* const dist = W.dist;
+    const uint32_t last_bin = W.dist_bins - 1u;
 #pragma unroll 1
     while ((tick < t || (tick == t && tseq < ev_seq)) && tick < horizon) {
 #pragma unroll 1
@@ -970,12 +985,24 @@ AF_FN void take_samples(State& W, double t, uint32_t ev_seq) {
             if (v > tbl_samp_max(W)[j]) tbl_samp_max(W)[j] = v;
             if (traced && (int32_t)nt < AF_L.trace_tick_cap)
                 AF_G.trace_series[(W.local * (uint64_t)n_series + (uint32_t)j) * (uint64_t)AF_L.trace_tick_cap + nt] = v;
-            if (band != nullptr && nt >= W.band_from) {
+            if ((band != nullptr || dist != nullptr) && nt >= W.band_from) {
                 const uint32_t p = tbl_band_prev(W)[j];
+                const int32_t s = dist != nullptr ? W.dist_slot[j] : -1;
+                if (s >= 0) {
+                    uint32_t* row = dist + (uint64_t)s * W.dist_series_words + (uint64_t)nt * W.dist_bins;
+                    uint32_t b1 = afr::gauge_bin(v); b1 = b1 < last_bin ? b1 : last_bin;
+                    if (nt == W.band_from) red_add_u32(row + b1, 1u);
+                    else {
+                        uint32_t b0 = afr::gauge_bin(p); b0 = b0 < last_bin ? b0 : last_bin;
+                        if (b0 != b1) { red_add_u32(row + b0, ~0u); red_add_u32(row + b1, 1u); }
+                    }
+                }
                 if (v != p) {
-                    uint64_t* row = band + (uint64_t)(1 + j) * stride + nt;
-                    red_add_u64(row, (uint64_t)v - (uint64_t)p);
-                    red_add_u64(row + sq, (uint64_t)v * v - (uint64_t)p * p);
+                    if (band != nullptr) {
+                        uint64_t* row = band + (uint64_t)(1 + j) * stride + nt;
+                        red_add_u64(row, (uint64_t)v - (uint64_t)p);
+                        red_add_u64(row + sq, (uint64_t)v * v - (uint64_t)p * p);
+                    }
                     tbl_band_prev(W)[j] = v;
                 }
             }
@@ -996,7 +1023,7 @@ AF_FN void band_stop(State& W) {
     AF_SHARED(&W);
     const int lane = lane_id();
     const uint64_t n = W.n_ticks, stride = W.band_stride, sq = (uint64_t)AF_L.n_series * stride;
-    if (n > W.band_from) {
+    if (n > W.band_from && W.band != nullptr) {
 #pragma unroll 1
         for (int32_t j = lane; j < AF_L.n_series; j += WARP) {
             const uint64_t p = tbl_band_prev(W)[j];
@@ -1007,8 +1034,19 @@ AF_FN void band_stop(State& W) {
         }
         if (lane == 0) red_add_u64(W.band + n, ~0ull);
     }
+    if (n > W.band_from && W.dist != nullptr) {       // distribution bands: the last emitted bin, a value of 0 included
+        const uint32_t last_bin = W.dist_bins - 1u;
+#pragma unroll 1
+        for (int32_t j = lane; j < AF_L.n_series; j += WARP) {
+            const int32_t s = W.dist_slot[j];
+            if (s < 0) continue;
+            uint32_t b = afr::gauge_bin(tbl_band_prev(W)[j]);
+            b = b < last_bin ? b : last_bin;
+            red_add_u32(W.dist + (uint64_t)s * W.dist_series_words + n * W.dist_bins + b, ~0u);
+        }
+    }
     w_sync();
-    W.band = nullptr;
+    W.band = nullptr; W.dist = nullptr;
     w_sync();
 }
 
@@ -1075,7 +1113,7 @@ AF_FN void load_params(State& W) {
     }
 #pragma unroll 1
     for (int32_t i = lane; i < AF_L.n_series; i += WARP) { tbl_samp_sum(W)[i] = 0; tbl_samp_max(W)[i] = 0; }
-    if (W.band != nullptr) for (int32_t i = lane; i < AF_L.n_series; i += WARP) tbl_band_prev(W)[i] = 0;
+    if (W.band != nullptr || W.dist != nullptr) for (int32_t i = lane; i < AF_L.n_series; i += WARP) tbl_band_prev(W)[i] = 0;
 #pragma unroll 1
     for (int32_t i = lane; i < AF_L.n_servers + 2; i += WARP) { InboxS b; b.head = b.tail = NIL; b.pending = 1; b.pad = 0; tbl_inbox(W)[i] = b; }
     w_sync();
@@ -1158,13 +1196,14 @@ AF_IN void run_replica(State& W, uint64_t local_index, const BandArgs& band) {
     W.traced = (int64_t)local_index < (int64_t)AF_L.trace_replicas ? 1u : 0u;
     W.band = nullptr; W.band_from = 0; W.band_stride = band.stride; W.band_prev_off = (uint32_t)band.prev_off;
     W.lat = nullptr; W.lat_from = 0; W.lat_window = band.lat_window;
-    if (band.stride || band.lat_window) {
+    W.dist = nullptr; W.dist_slot = band.dist_slot; W.dist_series_words = band.dist_series_words; W.dist_bins = band.dist_bins;
+    if (band.stride || band.lat_window || band.dist_rows) {
         const uint64_t i = W.replica - band.first;
         const uint32_t g = i < band.n ? band.group[i] : band.groups;
-        if (band.stride) {
-            W.band = band.rows + (uint64_t)g * band.group_words;
-            W.band_from = AF_G.redo_list ? band.from[local_index] : 0u;  // a re-run continues where the lane pass stopped
-        }
+        if (band.stride || band.dist_rows)                           // a re-run continues where the lane pass stopped
+            W.band_from = AF_G.redo_list ? band.from[local_index] : 0u;
+        if (band.stride) W.band = band.rows + (uint64_t)g * band.group_words;
+        if (band.dist_rows) W.dist = band.dist_rows + (uint64_t)g * band.dist_group_words;
         if (band.lat_window) {
             W.lat = band.lat_rows + (uint64_t)g * band.lat_windows * afr::LAT_ROW;
             W.lat_from = AF_G.redo_list ? band.lat_from[local_index] : 0u;
@@ -1235,7 +1274,7 @@ AF_IN void run_replica(State& W, uint64_t local_index, const BandArgs& band) {
         if (W.flags & STOP_FLAGS) break;
     }
     W.n_events = n_events;
-    if (W.band != nullptr && (W.flags & STOP_FLAGS)) band_stop(W);   // before the frozen ticks to the horizon
+    if ((W.band != nullptr || W.dist != nullptr) && (W.flags & STOP_FLAGS)) band_stop(W);   // before the frozen ticks to the horizon
     take_samples(W, W.horizon, 0u);                   // ticks strictly before the horizon
     write_back(W);
 }

@@ -91,11 +91,11 @@ __global__ void AF_LAUNCH_BOUNDS af_sim_kernel(const afc::BandArgs band) {
 // same kernel also accumulating the per-tick / per-window latency bands of the uploaded groups (af_run picks the one
 // the band options ask for); <false, false> is the kernel without them.  kLean: the loop without spikes, outages,
 // traces, the general edge sampler and the endpoint draw (af_run picks it when aflh::lean_launch says the launch can
-// reach none of them).
+// reach none of them).  kDist: the per-tick distribution bands of the selected series too (af_dist_bands_configure).
 #ifndef AF_LANE_MAX_THREADS
 #define AF_LANE_MAX_THREADS 384
 #endif
-template <bool kSampled = false, bool kLatency = false, bool kLean = false>
+template <bool kSampled = false, bool kLatency = false, bool kLean = false, bool kDist = false>
 __global__ void __launch_bounds__(AF_LANE_MAX_THREADS, 1) af_lane_kernel() {
     const afl::Cfg& C = afl::c_cfg;
     const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
@@ -108,7 +108,7 @@ __global__ void __launch_bounds__(AF_LANE_MAX_THREADS, 1) af_lane_kernel() {
     m.g128 = gs + lane * 16u;
     m.g64 = gs + (size_t)C.gn128 * afl::STRIDE128 + lane * 8u;
     m.g32 = gs + (size_t)C.gn128 * afl::STRIDE128 + (size_t)C.gn64 * afl::STRIDE64 + lane * 4u;
-    afl::run_lane<kSampled, kLatency, kLean>(m,
+    afl::run_lane<kSampled, kLatency, kLean, kDist>(m,
         [&]() -> uint64_t {
             const unsigned long long k = atomicAdd(C.work_counter, 1ull);
             return k < C.n_replicas ? (uint64_t)C.order[k] : ~0ull;
@@ -135,6 +135,22 @@ __global__ void af_band_scan_kernel(uint64_t* __restrict__ rows, uint64_t n_rows
         x += carry;
         if (k < n_ticks) r[k] = x;
         carry = __shfl_sync(0xFFFFFFFFu, x, 31);
+    }
+}
+
+// per-tick distribution bands: the difference rows -> per-tick bin counts, in place.  One thread per (group, series, bin)
+// of the n_rows = groups x series rows, a running u32 carry down the ticks; the threads of a warp read consecutive bins
+// of one tick row (coalesced).  u32 modular arithmetic: exact whatever order the REDs landed in, as a bin count stays
+// below 2^32 (a group holds fewer replicas than that).
+__global__ void af_dist_scan_kernel(uint32_t* __restrict__ rows, uint64_t n_rows, uint32_t n_bins, uint64_t series_words,
+                                    uint64_t n_ticks) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_rows * n_bins) return;
+    uint32_t* r = rows + (i / n_bins) * series_words + (i % n_bins);
+    uint32_t carry = 0;
+    for (uint64_t k = 0; k < n_ticks; ++k) {
+        carry += r[k * n_bins];
+        r[k * n_bins] = carry;
     }
 }
 
@@ -384,6 +400,12 @@ struct af_engine {
     int32_t band_sampled = 1, lat_window = 0;
     DevBuf d_lat, d_lat_from;
     bool last_lat = false; uint32_t last_lat_groups = 0; uint64_t last_lat_windows = 0;
+    // af_dist_bands_configure: the selected series (empty: per-tick distribution bands off), af_run's table of each
+    // series' slot (-1: not selected) and the rows over the groups of af_bands_upload
+    std::vector<int32_t> h_dist_series, h_dist_slot;
+    DevBuf d_dist_slot, d_dist;
+    bool last_dist = false; uint32_t last_dist_groups = 0, last_dist_ticks = 0, last_dist_bins = 0, last_dist_n = 0;
+    uint64_t last_dist_series_words = 0;
 
     int fail(int code, const std::string& m) { err = m; return code; }
     int cuda_fail(cudaError_t e, const char* what) {
@@ -457,7 +479,8 @@ void af_engine_destroy(af_engine* e) {
                       &e->d_stats, &e->d_sent, &e->d_dropped, &e->d_hist, &e->d_thr, &e->d_ssum, &e->d_smax,
                       &e->d_tclk, &e->d_tser, &e->d_tcnt, &e->d_counter, &e->d_htot,
                       &e->d_okey, &e->d_oidx, &e->d_order, &e->d_okey64, &e->d_sort_tmp,
-                      &e->d_band_group, &e->d_band, &e->d_band_from, &e->d_lat, &e->d_lat_from};
+                      &e->d_band_group, &e->d_band, &e->d_band_from, &e->d_lat, &e->d_lat_from,
+                      &e->d_dist_slot, &e->d_dist};
     for (DevBuf* b : bufs) b->release();
     cudaEventDestroy(e->ev_begin); cudaEventDestroy(e->ev_sim); cudaEventDestroy(e->ev_end);
     cudaStreamDestroy(e->stream);
@@ -625,6 +648,34 @@ static int lat_check(af_engine* e, uint64_t n_groups) {
     return AF_OK;
 }
 
+// the distribution bands' series and rows for `n_groups` groups of the current scenario, options and sweep
+// (afh::dist_series_check, afh::dist_bands_fit); sets the tick count and bins per tick row
+static int dist_check(af_engine* e, uint64_t n_groups, uint32_t& ticks, uint32_t& bins) {
+    std::string why;
+    if (!afh::dist_series_check(e->sc, e->h_dist_series.data(), (int32_t)e->h_dist_series.size(), why)
+        || !afh::dist_bands_fit(e->sc, e->opt, e->band_swept_ram, e->band_swept_server, n_groups, e->h_dist_series.size(),
+                                e->mem_total, ticks, bins, why))
+        return e->fail(AF_ERR_INVALID, why);
+    return AF_OK;
+}
+
+int af_dist_bands_configure(af_engine* e, const int32_t* series, int32_t n) {
+    if (!e) return AF_ERR_INVALID;
+    if (n < 0) return e->fail(AF_ERR_INVALID, "distribution bands: negative series count");
+    if (!series || n == 0) { e->h_dist_series.clear(); return AF_OK; }
+    if (!e->have_scenario) return e->fail(AF_ERR_STATE, "af_dist_bands_configure before af_scenario_upload");
+    std::vector<int32_t> old;
+    old.swap(e->h_dist_series);
+    e->h_dist_series.assign(series, series + n);
+    uint32_t ticks = 0, bins = 0;
+    std::string why;
+    int rc = AF_OK;
+    if (!afh::dist_series_check(e->sc, series, n, why)) rc = e->fail(AF_ERR_INVALID, why);
+    else if (e->band_groups > 0) rc = dist_check(e, e->band_groups, ticks, bins);     // the uploaded groups
+    if (rc) e->h_dist_series.swap(old);
+    return rc;
+}
+
 int af_bands_configure(af_engine* e, const AfBandOptions* opt) {
     if (!e || !opt) return AF_ERR_INVALID;
     if (opt->latency_window_s != 0) {
@@ -663,6 +714,8 @@ int af_bands_upload(af_engine* e, const uint32_t* group_of, uint64_t n, uint64_t
         if ((rc = band_check(e, largest_group(group_of, n)))) return rc;
     }
     if (e->lat_window && (rc = lat_check(e, n_groups))) return rc;
+    uint32_t bins = 0;
+    if (!e->h_dist_series.empty() && (rc = dist_check(e, n_groups, ticks, bins))) return rc;
     e->h_band_group.assign(group_of, group_of + n);
     if ((rc = upload_vec(e, e->d_band_group, e->h_band_group, "band groups"))) return rc;
     AF_CUDA(e, cudaStreamSynchronize(e->stream), "band groups H2D");
@@ -766,8 +819,19 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
     const uint64_t band_ticks = ticks32, band_stride = band_ticks + 1;
     const uint64_t band_group_words = (1 + 2 * (uint64_t)L.n_series) * band_stride;
     const uint64_t band_words = bands ? ((uint64_t)e->band_groups + 1) * band_group_words : 0;
+    // ---- per-tick distribution bands: (groups + 1) x n_dist x (ticks + 1) x bins u32 -----------------------------------
+    const bool dist = e->band_groups > 0 && !e->h_dist_series.empty();
+    uint32_t dist_ticks = 0, dist_bins = 0;
+    if (dist && (rc = dist_check(e, e->band_groups, dist_ticks, dist_bins))) return rc;
+    const uint64_t dist_n = dist ? e->h_dist_series.size() : 0;
+    const uint64_t dist_series_words = ((uint64_t)dist_ticks + 1) * dist_bins, dist_group_words = dist_n * dist_series_words;
+    const uint64_t dist_words = dist ? ((uint64_t)e->band_groups + 1) * dist_group_words : 0;
+    if (dist) {
+        e->h_dist_slot.assign((size_t)L.n_series, -1);
+        for (uint64_t s = 0; s < dist_n; ++s) e->h_dist_slot[(size_t)e->h_dist_series[s]] = (int32_t)s;
+    }
     afc::BandArgs band = {};
-    if (bands) {
+    if (bands || dist) {
         band.prev_off = L.warp_bytes;                       // the warp engine: each series' last emitted value, behind its tables
         L.warp_bytes += afc::align_up(4 * L.n_series, 16);
     }
@@ -805,6 +869,11 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
                                           : (lat ? af_lane_kernel<false, true, true> : af_lane_kernel<false, false, true>))
                                  : (bands ? (lat ? af_lane_kernel<true, true> : af_lane_kernel<true, false>)
                                           : (lat ? af_lane_kernel<false, true> : af_lane_kernel<false, false>));
+    if (dist)
+        lane_kernel = lean ? (bands ? (lat ? af_lane_kernel<true, true, true, true> : af_lane_kernel<true, false, true, true>)
+                                    : (lat ? af_lane_kernel<false, true, true, true> : af_lane_kernel<false, false, true, true>))
+                           : (bands ? (lat ? af_lane_kernel<true, true, false, true> : af_lane_kernel<true, false, false, true>)
+                                    : (lat ? af_lane_kernel<false, true, false, true> : af_lane_kernel<false, false, false, true>));
     if (lane) {
         lsmem = (size_t)lane_warps * (size_t)C.warp_bytes;
         AF_CUDA(e, cudaFuncSetAttribute(lane_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lsmem), "smem attribute");
@@ -850,9 +919,11 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
         AF_CUDA(e, e->d_tser.ensure(ntr * (uint64_t)L.n_series * (uint64_t)L.trace_tick_cap * 4 + 4), "trace series");
     }
     AF_CUDA(e, e->d_tcnt.ensure((ntr ? ntr : 1) * 8), "trace counts");
-    if (bands) {
-        AF_CUDA(e, e->d_band.ensure(band_words * 8), "band rows");
-        AF_CUDA(e, e->d_band_from.ensure(n * 4), "band stop ticks");
+    if (bands) AF_CUDA(e, e->d_band.ensure(band_words * 8), "band rows");
+    if (bands || dist) AF_CUDA(e, e->d_band_from.ensure(n * 4), "band stop ticks");
+    if (dist) {
+        AF_CUDA(e, e->d_dist.ensure(dist_words * 4), "distribution band rows");
+        if ((rc = upload_vec(e, e->d_dist_slot, e->h_dist_slot, "distribution band series"))) return rc;
     }
     if (lat) {
         AF_CUDA(e, e->d_lat.ensure(lat_words * 8), "latency band rows");
@@ -900,7 +971,12 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
     G.redo_list = redo ? (const uint32_t*)e->d_redo_list.p : nullptr;
     G.redo_count = redo ? (const uint32_t*)e->d_redo_count.p : nullptr;
     G.seed = seed; G.replica_begin = begin; G.n_replicas = n;
-    if (bands || lat) { band.group = (const uint32_t*)e->d_band_group.p; band.first = e->band_first; band.n = e->h_band_group.size(); band.groups = e->band_groups; }
+    if (bands || lat || dist) { band.group = (const uint32_t*)e->d_band_group.p; band.first = e->band_first; band.n = e->h_band_group.size(); band.groups = e->band_groups; }
+    if (dist) {
+        band.from = (const uint32_t*)e->d_band_from.p;
+        band.dist_rows = (uint32_t*)e->d_dist.p; band.dist_slot = (const int32_t*)e->d_dist_slot.p;
+        band.dist_group_words = dist_group_words; band.dist_series_words = dist_series_words; band.dist_bins = dist_bins;
+    }
     if (bands) {
         band.rows = (uint64_t*)e->d_band.p; band.from = (const uint32_t*)e->d_band_from.p;
         band.group_words = band_group_words; band.stride = (uint32_t)band_stride;
@@ -923,7 +999,13 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
         C.work_counter = (unsigned long long*)e->d_counter2.p;
         C.order = G.order;
         C.seed = seed; C.replica_begin = begin; C.n_replicas = n;
-        if (bands || lat) { C.band_group = band.group; C.band_first = band.first; C.band_n = band.n; C.band_groups = (int32_t)e->band_groups; }
+        if (bands || lat || dist) { C.band_group = band.group; C.band_first = band.first; C.band_n = band.n; C.band_groups = (int32_t)e->band_groups; }
+        if (dist) {
+            C.band_from = (uint32_t*)e->d_band_from.p;
+            C.dist_rows = band.dist_rows; C.dist_slot = band.dist_slot;
+            C.dist_group_words = dist_group_words; C.dist_series_words = dist_series_words;
+            C.dist_n = (int32_t)dist_n; C.dist_bins = (int32_t)dist_bins;
+        }
         if (bands) {
             C.band_rows = band.rows; C.band_from = (uint32_t*)e->d_band_from.p;
             C.band_group_words = band_group_words; C.band_stride = (int32_t)band_stride;
@@ -949,6 +1031,7 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
     if (L.collect_thr) AF_CUDA(e, cudaMemsetAsync(e->d_thr.p, 0, n * (uint64_t)L.horizon_s * 4, e->stream), "memset thr");
     if (bands) AF_CUDA(e, cudaMemsetAsync(e->d_band.p, 0, band_words * 8, e->stream), "memset band rows");
     if (lat) AF_CUDA(e, cudaMemsetAsync(e->d_lat.p, 0, lat_words * 8, e->stream), "memset latency band rows");
+    if (dist) AF_CUDA(e, cudaMemsetAsync(e->d_dist.p, 0, dist_words * 4, e->stream), "memset distribution band rows");
     {   // the pull order: (work, local index) heaviest first; then the first wave grouped by estimate
         uint32_t* key = (uint32_t*)e->d_okey.p; uint32_t* idx = (uint32_t*)e->d_oidx.p; uint32_t* order = (uint32_t*)e->d_order.p;
         uint64_t* key64 = (uint64_t*)e->d_okey64.p;
@@ -991,6 +1074,13 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
         AF_CUDA(e, cudaGetLastError(), "af_band_scan_kernel launch");
         e->launches += 1;
     }
+    if (dist) {       // the fetched groups' rows -> per-tick bin counts
+        const uint64_t rows = (uint64_t)e->band_groups * dist_n, threads = rows * dist_bins;
+        af_dist_scan_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, e->stream>>>((uint32_t*)e->d_dist.p, rows, dist_bins,
+                                                                                     dist_series_words, dist_ticks);
+        AF_CUDA(e, cudaGetLastError(), "af_dist_scan_kernel launch");
+        e->launches += 1;
+    }
     if (L.collect_hist) {
         unsigned blocks = (unsigned)((n * 32 + 255) / 256);
         af_percentile_kernel<<<blocks, 256, 0, e->stream>>>((const uint32_t*)e->d_hist.p, (AfReplicaStats*)e->d_stats.p, n);
@@ -1003,6 +1093,8 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
     e->last_bands = bands; e->last_band_groups = e->band_groups; e->last_band_ticks = (uint32_t)band_ticks;
     e->last_band_stride = band_stride;
     e->last_lat = lat; e->last_lat_groups = e->band_groups; e->last_lat_windows = lat_windows;
+    e->last_dist = dist; e->last_dist_groups = e->band_groups; e->last_dist_ticks = dist_ticks; e->last_dist_bins = dist_bins;
+    e->last_dist_n = (uint32_t)dist_n; e->last_dist_series_words = dist_series_words;
     return AF_OK;
 }
 
@@ -1197,6 +1289,21 @@ int af_fetch_latency_bands(af_engine* e, uint64_t* hist, uint64_t* sum_hi, uint6
         if (sum_lo) AF_CUDA(e, cudaMemcpy2DAsync(sum_lo + g * cap_windows, 8, gb + B + 1, R * 8, 8, k, cudaMemcpyDeviceToHost, e->stream),
                             "latency band sums D2H");
     }
+    return af_sync(e);
+}
+
+int af_fetch_dist_bands(af_engine* e, uint32_t* out, uint64_t cap_ticks, uint64_t* n_ticks, uint32_t* n_bins) {
+    if (!e || !n_ticks || !n_bins) return AF_ERR_INVALID;
+    if (!e->ran) return e->fail(AF_ERR_STATE, "fetch before af_run");
+    if (!e->last_dist) return e->fail(AF_ERR_STATE, "the last run collected no distribution bands (af_dist_bands_configure, af_bands_upload)");
+    AF_CUDA(e, cudaSetDevice(e->device), "cudaSetDevice");
+    const uint64_t T = e->last_dist_ticks, B = e->last_dist_bins, rows = (uint64_t)e->last_dist_groups * e->last_dist_n;
+    const uint64_t k = T < cap_ticks ? T : cap_ticks;
+    *n_ticks = T; *n_bins = (uint32_t)B;
+    if (!out || !k) return AF_OK;
+    // row (g, s) of the device is (T + 1) tick rows of B bins; the caller's holds cap_ticks of them
+    AF_CUDA(e, cudaMemcpy2DAsync(out, cap_ticks * B * 4, e->d_dist.p, e->last_dist_series_words * 4, k * B * 4, rows,
+                                 cudaMemcpyDeviceToHost, e->stream), "distribution bands D2H");
     return af_sync(e);
 }
 

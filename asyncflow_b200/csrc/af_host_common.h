@@ -170,6 +170,47 @@ inline bool band_sumsq_fits(uint64_t group, uint64_t bound) {
     return (unsigned __int128)group * bound * bound < ((unsigned __int128)1 << 64);
 }
 
+// Per-tick distribution bands (DESIGN.md §3.7).  The series af_dist_bands_configure selects, by their af_fetch_sampled
+// index: each in range, sampled by the scenario, listed once.
+inline bool dist_series_check(const AfScenario& s, const int32_t* series, int32_t n, std::string& why) {
+    const int32_t ns3 = 3 * s.n_servers, n_series = ns3 + s.n_edges;
+    std::vector<char> seen((size_t)n_series, 0);
+    for (int32_t i = 0; i < n; ++i) {
+        const int32_t j = series[i];
+        const char* bad = nullptr;
+        if (j < 0 || j >= n_series) bad = "is not a sampled series of the scenario (index out of range)";
+        else if (j < ns3 ? (s.metrics_mask & 7u) != 7u : (s.metrics_mask & AF_METRIC_EDGE_CONN) == 0) bad = "is not sampled by the scenario";
+        else if (seen[(size_t)j]) bad = "is listed twice";
+        if (bad) {
+            char b[200];
+            snprintf(b, sizeof b, "distribution bands: series[%d] = %d %s (%d series)", i, j, bad, n_series);
+            why = b;
+            return false;
+        }
+        seen[(size_t)j] = 1;
+    }
+    return true;
+}
+// The checks af_dist_bands_configure, af_bands_upload and af_run apply to distribution bands of n_dist series over
+// n_groups groups: fewer than BAND_TICK_LIMIT ticks, and rows of (n_groups + 1) x n_dist x (ticks + 1) x bins u32 the
+// device (mem_total bytes) can hold.  bins = gauge_bin(bound) + 1 for the band_gauge_bound of the scenario, options and
+// sweep.  Sets ticks and bins.
+inline bool dist_bands_fit(const AfScenario& s, const AfOptions& o, uint64_t swept_ram, int32_t swept_server, uint64_t n_groups,
+                           uint64_t n_dist, uint64_t mem_total, uint32_t& ticks, uint32_t& bins, std::string& why) {
+    std::string what;
+    const uint64_t bound = band_gauge_bound(s, o, swept_ram, swept_server, what);
+    bins = afr::gauge_bin((uint32_t)(bound < 0xFFFFFFFFull ? bound : 0xFFFFFFFFull)) + 1u;
+    if (!band_ticks_fit(s, ticks, why)) { why = "distribution " + why; return false; }
+    const unsigned __int128 bytes = ((unsigned __int128)n_groups + 1) * n_dist * ((unsigned __int128)ticks + 1) * bins * 4u;
+    if (bytes <= (unsigned __int128)mem_total) return true;
+    char b[320];
+    snprintf(b, sizeof b, "distribution bands: %llu groups x %llu series x %u ticks x %u bins (bound on a gauge %llu: %s) need "
+             "%.3g GB of rows, more than the device's %.3g GB", (unsigned long long)n_groups, (unsigned long long)n_dist,
+             ticks, bins, (unsigned long long)bound, what.c_str(), (double)bytes / 1e9, (double)mem_total / 1e9);
+    why = b;
+    return false;
+}
+
 inline void make_layout(const AfScenario& s, const AfOptions& o, int32_t n_sweep_cols, afc::Layout& L) {
     L.n_edges = s.n_edges; L.n_servers = s.n_servers; L.n_endpoints = s.n_endpoints; L.n_steps = s.n_steps;
     L.n_lb_edges = s.n_lb_edges; L.lb_algo = s.lb_algo; L.gen_edge = s.gen_edge; L.client_edge = s.client_edge;

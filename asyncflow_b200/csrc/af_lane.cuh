@@ -180,6 +180,13 @@ struct Cfg {
     // stopped replica added (the warp-per-replica pass adds the rest).
     uint64_t* lat_rows; uint32_t* lat_from;
     int32_t lat_window, lat_windows;
+    // per-tick distribution bands (run_lane<*, *, *, true> only; DESIGN.md §3.7), over the groups of band_group: the
+    // count of bin b of selected series s at tick row k of group g is the u32 at dist_rows + g * dist_group_words +
+    // s * dist_series_words + k * dist_bins + b (difference rows over k until af_dist_scan_kernel).  dist_slot[j] = s
+    // for a selected series j, -1 for the others.  band_from is shared with the per-tick bands.
+    uint32_t* dist_rows; const int32_t* dist_slot;
+    uint64_t dist_group_words, dist_series_words;
+    int32_t dist_n, dist_bins;
 };
 
 
@@ -295,6 +302,7 @@ struct St {
     uint64_t n_events;
     double lat_sum, lat_sumsq, lat_min, lat_max;
     uint64_t* band;                             // run_lane<true, *>: the replica's group's difference rows
+    uint32_t dist_g;                            // run_lane<*, *, *, true>: the replica's group (distribution bands)
 };
 
 // flags that end a replica early (its partial results are written back with the flag set)
@@ -549,7 +557,25 @@ AFL_IN bool gen_next_gap(St& W, double& gap) {
 // Per-tick bands (kBands) ride on the same moment: a change from v to v + delta with n_ticks ticks taken before it adds
 // delta to the series at every tick k >= n_ticks, so the sums over a group's replicas are difference arrays -- one RED
 // of delta (and of (v + delta)^2 - v^2) at index n_ticks per change, one prefix scan after the launch (DESIGN.md §3.4).
-template <bool kBands>
+// Distribution bands (kDist) too, over (tick, value bin): from tick n_ticks on the replica leaves bin(v) for
+// bin(v + delta) -- one RED of -1 and one of +1 at row n_ticks of a selected series, none when the bin stays (§3.7).
+// The replica's group is W.dist_g (a u32 register; a local of run_lane's would move the SASS of the kernels without).
+AFL_IN uint32_t* dist_row(uint32_t dg, int32_t s, uint32_t k) {
+    return AFL_C.dist_rows + (uint64_t)dg * AFL_C.dist_group_words + (uint64_t)(uint32_t)s * AFL_C.dist_series_words
+           + (uint64_t)k * (uint32_t)AFL_C.dist_bins;
+}
+AFL_IN uint32_t dist_bin(uint32_t v) {              // (values above the launch's gauge bound cannot occur: clamped anyway)
+    const uint32_t b = afr::gauge_bin(v), last = (uint32_t)AFL_C.dist_bins - 1u;
+    return b < last ? b : last;
+}
+AFL_IN int32_t dist_slot(int32_t j) {
+#if AFL_DEVICE
+    return __ldg(AFL_C.dist_slot + j);
+#else
+    return AFL_C.dist_slot[j];
+#endif
+}
+template <bool kBands, bool kDist>
 AFL_IN void gauge_touch(const St& W, const Mem& m, int32_t j, uint32_t v_old, int32_t delta) {
     red_add64(g64p(m, AFL_C.gi_acc + j), (uint64_t)(int64_t)delta * (uint64_t)W.n_ticks);
     if constexpr (kBands) {
@@ -558,6 +584,17 @@ AFL_IN void gauge_touch(const St& W, const Mem& m, int32_t j, uint32_t v_old, in
         red_add64(row, (uint64_t)(int64_t)delta);
         red_add64(row + (uint64_t)AFL_C.n_series * (uint64_t)AFL_C.band_stride, v1 * v1 - v0 * v0);
     }
+    if constexpr (kDist) {
+        const int32_t s = dist_slot(j);
+        if (s >= 0) {
+            const uint32_t b0 = dist_bin(v_old), b1 = dist_bin(v_old + (uint32_t)delta);
+            if (b0 != b1) {
+                uint32_t* row = dist_row(W.dist_g, s, W.n_ticks);
+                red_add32(row + b0, ~0u);
+                red_add32(row + b1, 1u);
+            }
+        }
+    }
     const int32_t dw = AFL_C.o32_dirty + (j >> 5);
     const uint32_t d = w32_ld(m, dw), bit = 1u << (j & 31);
     if (!(d & bit)) {
@@ -565,22 +602,22 @@ AFL_IN void gauge_touch(const St& W, const Mem& m, int32_t j, uint32_t v_old, in
         w32_st(m, dw, d | bit);
     }
 }
-template <bool kBands>
+template <bool kBands, bool kDist>
 AFL_IN void conn_add(const St& W, const Mem& m, uint32_t edge, int32_t delta) {
     const int32_t pw = AFL_C.o32_conn + (int32_t)edge;
     const uint32_t v = w32_ld(m, pw);
-    if (AFL_C.metrics_mask & AF_METRIC_EDGE_CONN) gauge_touch<kBands>(W, m, 3 * AFL_C.n_servers + (int32_t)edge, v, delta);
+    if (AFL_C.metrics_mask & AF_METRIC_EDGE_CONN) gauge_touch<kBands, kDist>(W, m, 3 * AFL_C.n_servers + (int32_t)edge, v, delta);
     w32_st(m, pw, v + (uint32_t)delta);
 }
 AFL_IN int32_t ib_word(uint32_t node, int32_t f) { return AFL_C.c_inbox + (int32_t)node * IB_WORDS + f; }      // cold
 AFL_IN int32_t sq_word(uint32_t sidx, int32_t f) { return AFL_C.c_srvq + (int32_t)sidx * SQ_WORDS + f; }       // cold
 AFL_IN int32_t sv_word(uint32_t sidx, int32_t f) { return AFL_C.o32_srv + (int32_t)sidx * SV_WORDS + f; }
 // field = SV_READY_Q / SV_IO_Q / SV_RAM_IN_USE (series 3 * sidx + 0 / 1 / 2)
-template <bool kBands>
+template <bool kBands, bool kDist>
 AFL_IN void srv_gauge_add(const St& W, const Mem& m, uint32_t sidx, int32_t field, int32_t delta) {
     const int32_t pw = sv_word(sidx, field);
     const int32_t v = i32_ld(m, pw);
-    if ((AFL_C.metrics_mask & 7u) == 7u) gauge_touch<kBands>(W, m, 3 * (int32_t)sidx + (field - SV_READY_Q), (uint32_t)v, delta);
+    if ((AFL_C.metrics_mask & 7u) == 7u) gauge_touch<kBands, kDist>(W, m, 3 * (int32_t)sidx + (field - SV_READY_Q), (uint32_t)v, delta);
     i32_st(m, pw, v + delta);
 }
 AFL_IN uint32_t gauge_value(const Mem& m, int32_t j) {
@@ -668,6 +705,26 @@ AFL_IN void lat_add(const St& W, uint32_t& lat_g, uint32_t done, double lat) {
 }
 AFL_IN void lat_stop(const St& W, uint32_t lat_g) {
     if (lat_g != LAT_OFF) AFL_C.lat_from[W.local] = W.completed;
+}
+
+// ---- per-tick distribution bands: the join and leave of the per-tick bands, over (tick, value bin) of the selected
+//      series.  A replica joins bin(0) = 0 of every selected series at tick 0 and, stopped, leaves the bin of its
+//      current value at its stop tick -- a value of 0 included (band_stop skips it: it adds nothing to a sum, but here
+//      the replica would stay in the count).  dist_start keeps the replica's group (lat_group's) in W.dist_g for
+//      gauge_touch.  One stop tick per replica in band_from, whichever kinds of bands are on.
+AFL_IN void dist_start(St& W) {
+    W.dist_g = lat_group(W);
+#pragma unroll 1
+    for (int32_t s = 0; s < AFL_C.dist_n; ++s) red_add32(dist_row(W.dist_g, s, 0u), 1u);
+}
+AFL_IN void dist_stop(const St& W, const Mem& m) {
+    const uint32_t n = W.n_ticks;
+#pragma unroll 1
+    for (int32_t j = 0; j < AFL_C.n_series; ++j) {
+        const int32_t s = dist_slot(j);
+        if (s >= 0) red_add32(dist_row(W.dist_g, s, n) + dist_bin(gauge_value(m, j)), ~0u);
+    }
+    AFL_C.band_from[W.local] = n;
 }
 
 // ---- Stores (mailboxes), Containers: as af_core.cuh ----------------------------------------------------
@@ -913,8 +970,10 @@ enum : uint32_t { A_NONE = 0, A_NODE, A_STEPS, A_SEND, A_TIMER };
 // `kLean`: the launch has no spikes, no outages, no traced replica, only normal and exponential edges and one endpoint
 // per server (aflh::lean_launch); the code for those features is left out of the loop, which does the same work in
 // the same order with fewer instructions to fetch.  <S, L, false> compiles to the same code as before kLean existed.
+// `kDist`: the per-tick distribution bands of the selected series (Cfg.dist_*) too; <S, L, Lean, false> compiles to
+// the same code as before kDist existed.
 // ---------------------------------------------------------------------------------------------------
-template <bool kSampled = false, bool kLatency = false, bool kLean = false, class NextFn, class ConvFn>
+template <bool kSampled = false, bool kLatency = false, bool kLean = false, bool kDist = false, class NextFn, class ConvFn>
 AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
     const Cfg& C = AFL_C;
     St W;
@@ -931,6 +990,7 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                 start_replica<kLean>(W, m, r);
                 if constexpr (kSampled) band_start(W);
                 if constexpr (kLatency) lat_g = lat_group(W);
+                if constexpr (kDist) dist_start(W);
                 // start order of the reference (simulation_runner.py:339-342, 301-336):
                 // spike timeline, outage timeline, generator, ..., collector
                 if (!kLean && C.n_spike > 0) {
@@ -1022,6 +1082,7 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
         // ---- phase: collector ticks that fall before this event ------------------------------------------------
         if constexpr (kSampled) { if (AFL_UNLIKELY(dead)) band_stop(W, m); }     // before the frozen ticks to the horizon
         if constexpr (kLatency) { if (AFL_UNLIKELY(dead)) lat_stop(W, lat_g); }
+        if constexpr (kDist) { if (AFL_UNLIKELY(dead)) dist_stop(W, m); }
         if (run && !is_item) {
             const double tick = W.tick_time;
             if (tick < t_ev || (tick == t_ev && W.tick_seq < ev_seq)) take_ticks<kLean>(W, m, t_ev, ev_seq);
@@ -1044,7 +1105,7 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
         if (names_request) rq_load(W, m, slot, t0, rid, pack);
         if (is_event) {
             if (kind == K_DELIVER) {                          // edge.py:110-116: the edge's timeout fired
-                conn_add<kSampled>(W, m, aux, -1);
+                conn_add<kSampled, kDist>(W, m, aux, -1);
                 const uint32_t meta = ro(C.edges + aux).meta;
                 pack += 1;                                     // record_hop(edge)
                 const uint32_t tk = (meta >> 3) & 3u;
@@ -1091,11 +1152,11 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                 consumer_get(W, m, NODE_CLIENT);
             } else if (kind == I_RAM_OK) {                     // the RAM get event is processed: the handler resumes
                 sidx = aux;
-                srv_gauge_add<kSampled>(W, m, sidx, SV_RAM_IN_USE, (int32_t)ep_total_ram(m, pk_ep(pack)));
+                srv_gauge_add<kSampled, kDist>(W, m, sidx, SV_RAM_IN_USE, (int32_t)ep_total_ram(m, pk_ep(pack)));
                 act = A_STEPS;
             } else if (kind == I_CPU_OK) {                     // the CPU get event is processed
                 sidx = aux;
-                if (pack & PK_WAIT) { pack &= ~PK_WAIT; srv_gauge_add<kSampled>(W, m, sidx, SV_READY_Q, -1); }
+                if (pack & PK_WAIT) { pack &= ~PK_WAIT; srv_gauge_add<kSampled, kDist>(W, m, sidx, SV_READY_Q, -1); }
                 pack |= PK_CORE;
                 act = A_STEPS;
             } else if (kind == I_CPU_PUT) {                    // waiters are re-examined, then the request goes on
@@ -1142,7 +1203,7 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                         go = false;
                     } else {
                         i32_st(m, sv_word(sidx, SV_RAM_FREE), i32_ld(m, sv_word(sidx, SV_RAM_FREE)) - (int32_t)total_ram);   // granted, and its get event would run next
-                        srv_gauge_add<kSampled>(W, m, sidx, SV_RAM_IN_USE, (int32_t)total_ram);
+                        srv_gauge_add<kSampled, kDist>(W, m, sidx, SV_RAM_IN_USE, (int32_t)total_ram);
                     }
                 }
                 if (go) act = A_STEPS;
@@ -1197,7 +1258,7 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                 if (st < ep.n_steps) {
                     const StepP sp = ro(C.steps + ep.step_begin + st);
                     if (sp.kind == AF_STEP_CPU) {
-                        if (pack & PK_IO) { pack &= ~PK_IO; srv_gauge_add<kSampled>(W, m, sidx, SV_IO_Q, -1); }
+                        if (pack & PK_IO) { pack &= ~PK_IO; srv_gauge_add<kSampled, kDist>(W, m, sidx, SV_IO_Q, -1); }
                         if (!(pack & PK_CORE)) {             // cpu_req = CPU.get(1); yield cpu_req
                             if (can_fuse(W) && i32_ld(m, sv_word(sidx, SV_CPU_FREE)) > 0 && q_empty(W, m, sq_word(sidx, SQ_CPUQ_HEAD))) {
                                 i32_st(m, sv_word(sidx, SV_CPU_FREE), i32_ld(m, sv_word(sidx, SV_CPU_FREE)) - 1);     // granted, and its get event would run next
@@ -1205,7 +1266,7 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                             } else {
                                 fifo_push(m, sq_word(sidx, SQ_CPUQ_HEAD), sq_word(sidx, SQ_CPUQ_TAIL), slot);
                                 W.n_waiting += 1;
-                                if (!cpu_walk(W, m, sidx, slot)) { pack |= PK_WAIT; srv_gauge_add<kSampled>(W, m, sidx, SV_READY_Q, 1); }   // not cpu_req.triggered
+                                if (!cpu_walk(W, m, sidx, slot)) { pack |= PK_WAIT; srv_gauge_add<kSampled, kDist>(W, m, sidx, SV_READY_Q, 1); }   // not cpu_req.triggered
                                 break;
                             }
                         }
@@ -1220,7 +1281,7 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                             nq_push(W, m, I_CPU_PUT, sidx, slot);
                             break;
                         }
-                        if (!(pack & PK_IO)) { pack |= PK_IO; srv_gauge_add<kSampled>(W, m, sidx, SV_IO_Q, 1); }
+                        if (!(pack & PK_IO)) { pack |= PK_IO; srv_gauge_add<kSampled, kDist>(W, m, sidx, SV_IO_Q, 1); }
                     }
                     const double dur = sp.c_dur >= 0 ? row_val(m, sp.c_dur) : sp.dur;
                     tm_t = W.now + dur; tm_payload = mk_payload(K_STEP_END, sidx, slot); tm_seq = W.seq++;
@@ -1238,10 +1299,10 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                     nq_push(W, m, I_CPU_PUT, sidx, slot);
                     break;
                 }
-                if (pack & PK_IO) { pack &= ~PK_IO; srv_gauge_add<kSampled>(W, m, sidx, SV_IO_Q, -1); }
+                if (pack & PK_IO) { pack &= ~PK_IO; srv_gauge_add<kSampled, kDist>(W, m, sidx, SV_IO_Q, -1); }
                 const uint32_t total_ram = ep.c_ram >= 0 ? (uint32_t)row_val(m, ep.c_ram) : ep.total_ram;
                 if (total_ram) {                             // yield RAM.put(total_ram): level rises NOW
-                    srv_gauge_add<kSampled>(W, m, sidx, SV_RAM_IN_USE, -(int32_t)total_ram);
+                    srv_gauge_add<kSampled, kDist>(W, m, sidx, SV_RAM_IN_USE, -(int32_t)total_ram);
                     i32_st(m, sv_word(sidx, SV_RAM_FREE), i32_ld(m, sv_word(sidx, SV_RAM_FREE)) + (int32_t)total_ram);
                     if (!can_fuse(W)) { nq_push(W, m, I_RAM_PUT, sidx, slot); break; }
                     if (AFL_UNLIKELY(!q_empty(W, m, sq_word(sidx, SQ_RAMQ_HEAD)))) ram_walk(W, m, sidx);   // the put event would run next: waiters, then forward
@@ -1337,7 +1398,7 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                     rq_release(W, m, slot);
                 } else {
                     rq_pack_set(W, m, slot, pack);              // (the one store of the record on the request's way out of a node)
-                    conn_add<kSampled>(W, m, edge, 1);
+                    conn_add<kSampled, kDist>(W, m, edge, 1);
                     double effective = transit;
                     if (!kLean && C.n_spike > 0) effective = transit + f64_ld(m, C.o64_spike + (int32_t)edge);   // spike read at SEND time (edge.py:94-106)
                     else effective = transit + 0.0;         // (-0.0 + 0.0 = +0.0, as with a spike table of zeros)

@@ -98,6 +98,18 @@ AF_HD int32_t hist_bin(double lat) {
     return idx < 0 ? 0 : (idx >= AF_HIST_BINS ? AF_HIST_BINS - 1 : idx);
 }
 
+// The distribution bands' bin of a gauge value (DESIGN.md §3.7): one bin per value below 64, then 16 log-linear bins per
+// octave (a bin is at most 1/16 of its lower edge wide).  results.gauge_bin_edges restates the edges in Python.
+AF_HD uint32_t gauge_bin(uint32_t v) {
+    if (v < 64u) return v;
+#if defined(__CUDA_ARCH__)
+    const uint32_t m = 31u - (uint32_t)__clz((int)v);
+#else
+    const uint32_t m = 31u - (uint32_t)__builtin_clz(v);
+#endif
+    return 64u + 16u * (m - 6u) + ((v >> (m - 4u)) & 15u);
+}
+
 // A latency in 32.32 fixed point: round-to-nearest-even(lat * 2^32) (the scaling by 2^32 is exact).  Per-window latency
 // bands add these as two u64 words, so their sums are exact in whatever order the additions land.  A window of a
 // group's latency bands is LAT_ROW words: AF_HIST_BINS bin counts, the sum's high word (u >> 32), its low word.

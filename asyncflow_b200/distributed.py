@@ -18,7 +18,7 @@ from dataclasses import dataclass
 import numpy as np
 
 from . import _capi as K
-from .results import SweepResults, hist_percentiles
+from .results import SweepResults, hist_percentiles, pad_dist_bins
 
 N_TOTALS = 8     # completed, generated, events, replicas, overflowed, ticks, reserved x2
 
@@ -98,24 +98,30 @@ def all_gather_summary(ints: np.ndarray, flts: np.ndarray, device: str | None = 
         per_rank_completed=[int(x) for x in tot[:, 0]])
 
 
-BAND_FIELDS = ("band_count", "band_sum", "band_sumsq", "lat_hist", "lat_sum_hi", "lat_sum_lo", "group_size")
+BAND_FIELDS = ("band_count", "band_sum", "band_sumsq", "lat_hist", "lat_sum_hi", "lat_sum_lo", "group_size", "dist_hist")
 
 
 def all_reduce_bands(res: SweepResults, device: str | None = None) -> SweepResults:
-    """Sum the band rows of ``res`` -- the per-tick sampled-metric bands, the per-window latency bands and the group
-    sizes a rank's shard holds -- over every rank, in place, with one all-reduce: afterwards each rank holds the
-    bands of the whole sweep, as :meth:`SweepResults.concatenate` of every rank's results would.  The unsigned sums
-    travel as int64; their modular addition gives the same bits.  Works without an initialised process group."""
+    """Sum the band rows of ``res`` -- the per-tick sampled-metric bands, the per-window latency bands, the per-tick
+    distribution bands and the group sizes a rank's shard holds -- over every rank, in place, with one all-reduce:
+    afterwards each rank holds the bands of the whole sweep, as :meth:`SweepResults.concatenate` of every rank's
+    results would.  The unsigned sums travel as int64; their modular addition gives the same bits.  Ranks may size
+    their distribution bins differently (each launch by its own rows): one all-reduce of the largest bin count comes
+    first, and every rank pads to it.  Works without an initialised process group."""
     import torch  # noqa: PLC0415
     import torch.distributed as dist  # noqa: PLC0415
 
-    present = [(k, getattr(res, k)) for k in BAND_FIELDS if getattr(res, k) is not None]
     world = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
-    if world == 1 or not present:
+    if world == 1 or not any(getattr(res, k) is not None for k in BAND_FIELDS):
         return res
+    dev = device or ("cuda" if dist.get_backend() == "nccl" else "cpu")
+    if res.dist_hist is not None:
+        b = torch.tensor([res.dist_hist.shape[-1]], dtype=torch.int64, device=dev)
+        dist.all_reduce(b, op=dist.ReduceOp.MAX)
+        res.dist_hist = pad_dist_bins(res.dist_hist, int(b.item()))
+    present = [(k, getattr(res, k)) for k in BAND_FIELDS if getattr(res, k) is not None]
     flat = np.concatenate([a.astype(np.uint64).view(np.int64).ravel() if a.dtype != np.int64 else a.ravel()
                            for _, a in present])
-    dev = device or ("cuda" if dist.get_backend() == "nccl" else "cpu")
     t = torch.from_numpy(flat).to(dev)
     dist.all_reduce(t, op=dist.ReduceOp.SUM)
     out = t.cpu().numpy()

@@ -35,6 +35,7 @@ class Engine:
         self._band_groups = self._run_band_groups = 0
         self._band_opt = K.AfBandOptions(1, 0)
         self._run_band_opt = (1, 0)
+        self._dist_n = self._run_dist_n = 0
 
     # ------------------------------------------------------------------ plumbing
     def _check(self, rc: int, what: str) -> None:
@@ -94,6 +95,7 @@ class Engine:
         self._n = int(replica_end) - int(replica_begin)
         self._run_band_groups = self._band_groups
         self._run_band_opt = (self._band_opt.sampled, self._band_opt.latency_window_s)
+        self._run_dist_n = self._dist_n
 
     def sync(self) -> None:
         self._check(self._lib.af_sync(self._h), "af_sync")
@@ -183,6 +185,28 @@ class Engine:
         opt = K.AfBandOptions(int(bool(sampled)), int(latency_window_s))
         self._check(self._lib.af_bands_configure(self._h, C.byref(opt)), "af_bands_configure")
         self._band_opt = opt
+
+    def configure_dist_bands(self, series) -> None:
+        """Per-tick distribution bands of the sampled series ``series`` (indices in the order of :meth:`sampled`; empty
+        or ``None``: off) over the uploaded groups from the next run on (:meth:`dist_bands`) --
+        ``af_dist_bands_configure``."""
+        s = np.ascontiguousarray([] if series is None else series, dtype=np.int32)
+        self._check(self._lib.af_dist_bands_configure(self._h, s.ctypes.data if s.size else None, int(s.size)),
+                    "af_dist_bands_configure")
+        self._dist_n = int(s.size)
+
+    def dist_bands(self) -> np.ndarray:
+        """Distribution bands of the last run: ``[G, n_dist, T, n_bins]`` u32 -- per group, selected series, tick and
+        value bin (``results.gauge_bin_edges``), the replicas that contribute the tick with a value in the bin
+        (``af_fetch_dist_bands``)."""
+        T, B = C.c_uint64(), C.c_uint32()
+        self._check(self._lib.af_fetch_dist_bands(self._h, None, 0, C.byref(T), C.byref(B)), "af_fetch_dist_bands")
+        rows = self._run_band_groups * self._run_dist_n
+        out = np.empty((self._run_band_groups, self._run_dist_n, T.value, B.value), dtype=np.uint32)
+        if rows and T.value:
+            self._check(self._lib.af_fetch_dist_bands(self._h, out.ctypes.data, T.value, C.byref(T), C.byref(B)),
+                        "af_fetch_dist_bands")
+        return out
 
     def latency_bands(self) -> tuple[np.ndarray, np.ndarray, np.ndarray]:
         """Latency bands of the last run: ``(hist [G, W, AF_HIST_BINS] u64, sum_hi [G, W] u64, sum_lo [G, W] u64)`` --

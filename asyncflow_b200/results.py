@@ -72,6 +72,46 @@ def hist_percentiles(hist: np.ndarray, q: float) -> np.ndarray:
     return out.reshape(h.shape[:-1])
 
 
+def gauge_bin_edges(n_bins: int) -> np.ndarray:
+    """Lower edges of the first ``n_bins`` value bins of the distribution bands (``af_dist_bands_configure``), ``[n_bins]``
+    int64: one bin per value below 64, then 16 log-linear bins per octave (the engine's ``afr::gauge_bin``).  Bin ``b``
+    holds the values in ``[edges[b], edges[b + 1])``."""
+    b = np.arange(int(n_bins), dtype=np.int64)
+    hi = np.maximum(b - 64, 0)
+    m = hi // 16 + 6                                          # the octave: index of the highest set bit
+    return np.where(b < 64, b, (16 + hi % 16) << np.maximum(m - 4, 0))
+
+
+def pad_dist_bins(hist: np.ndarray, n_bins: int) -> np.ndarray:
+    """Distribution-band counts ``[..., b]`` widened to ``n_bins`` bins with zeros.  A launch sizes its bins by the largest
+    value it can see (the request capacity or the largest ``ram_mb`` of its own sweep rows), so shards of one sweep may
+    differ in their bin count; the edges (:func:`gauge_bin_edges`) are the same for all, so the extra bins are empty."""
+    b = hist.shape[-1]
+    if b == n_bins:
+        return hist
+    if b > n_bins:
+        msg = f"cannot narrow {b} distribution bins to {n_bins}"
+        raise ValueError(msg)
+    out = np.zeros(hist.shape[:-1] + (int(n_bins),), dtype=hist.dtype)
+    out[..., :b] = hist
+    return out
+
+
+def series_index(flat: FlatScenario, key: Any, entity_id: str) -> int | None:
+    """Row of ``(key, entity_id)`` -- as ``ResultsAnalyzer.get_series`` takes them -- in the sampled series, or ``None``
+    when the scenario does not sample that metric."""
+    name = str(getattr(key, "value", key))
+    en = set(flat.enabled_metrics)
+    if name in SERVER_SERIES:
+        i = list(flat.server_ids).index(entity_id)
+        return 3 * i + SERVER_SERIES.index(name) if all(m in en for m in SERVER_SERIES) else None
+    if name == EDGE_SERIES:
+        e = list(flat.edge_ids).index(entity_id)
+        return 3 * flat.n_servers + e if EDGE_SERIES in en else None
+    msg = f"unknown sampled metric {name!r}"
+    raise KeyError(msg)
+
+
 def fixed32_mean(sum_hi: np.ndarray, sum_lo: np.ndarray, n: np.ndarray) -> np.ndarray:
     """Mean latency from the two words of a 32.32 fixed-point latency sum (``sum_hi * 2**32 + sum_lo``) over ``n``
     completions; NaN where ``n == 0``."""
@@ -241,6 +281,11 @@ class SweepResults:
         self.lat_sum_hi: np.ndarray | None = None
         self.lat_sum_lo: np.ndarray | None = None
         self.group_size: np.ndarray | None = None
+        # per-tick distribution bands (SweepRunner(dist_series=[...])): per group g, selected series s (dist_series[s],
+        # a (metric, entity_id) key), tick k and value bin b (gauge_bin_edges), the replicas that contribute the tick
+        # with a value in the bin -- [G, n_dist, T, n_bins] u32
+        self.dist_series: list[tuple[str, str]] = []
+        self.dist_hist: np.ndarray | None = None
 
     def __len__(self) -> int:
         return int(self.stats.shape[0])
@@ -337,6 +382,7 @@ class SweepResults:
         out.lat_window_s, out.lat_hist, out.lat_sum_hi, out.lat_sum_lo = (self.lat_window_s, self.lat_hist,
                                                                           self.lat_sum_hi, self.lat_sum_lo)
         out.group_size = self.group_size
+        out.dist_series, out.dist_hist = self.dist_series, self.dist_hist
         return out
 
     def bands(self, key: Any, entity_id: str) -> dict[str, np.ndarray]:
@@ -346,16 +392,7 @@ class SweepResults:
     def series_index(self, key: Any, entity_id: str) -> int | None:
         """Row of ``(key, entity_id)`` -- as ``ResultsAnalyzer.get_series`` takes them -- in the sampled series, or
         ``None`` when the scenario does not sample that metric."""
-        name = str(getattr(key, "value", key))
-        en = set(self.flat.enabled_metrics)
-        if name in SERVER_SERIES:
-            i = list(self.flat.server_ids).index(entity_id)
-            return 3 * i + SERVER_SERIES.index(name) if all(m in en for m in SERVER_SERIES) else None
-        if name == EDGE_SERIES:
-            e = list(self.flat.edge_ids).index(entity_id)
-            return 3 * self.flat.n_servers + e if EDGE_SERIES in en else None
-        msg = f"unknown sampled metric {name!r}"
-        raise KeyError(msg)
+        return series_index(self.flat, key, entity_id)
 
     def group_bands(self, key: Any, entity_id: str, level: float = 0.95) -> dict[str, np.ndarray]:
         """Per group and tick, over the group's replicas, of one sampled series (``SweepRunner(bands=...)``):
@@ -384,6 +421,58 @@ class SweepResults:
             half = NormalDist().inv_cdf(0.5 + level / 2.0) * std / np.sqrt(n)
         return {"t": np.arange(T) * self.flat.sample_period, "n": self.band_count, "mean": mean, "std": std,
                 "lo": mean - half, "hi": mean + half}
+
+    def group_dist(self, key: Any, entity_id: str, q=(0.05, 0.25, 0.5, 0.75, 0.95),
+                   at_least: int | None = None) -> dict[str, Any]:
+        """Per group and tick, the distribution over the group's replicas of one sampled series the sweep selected
+        (``SweepRunner(dist_series=[...])``): ``{"t", "n", "min", "max", "q", "p_at_least"}``.  ``t`` (``[T]``,
+        seconds) is the axis of :meth:`group_bands`; ``n`` (``[G, T]``) the replicas that contribute the tick; ``q``
+        (``[G, len(q), T]``) each quantile as ``numpy.quantile(..., method="inverted_cdf")`` gives it -- the smallest value
+        whose cumulative count reaches ``q * n`` -- reported, like ``min`` and ``max`` (``[G, T]``), as the lower edge of
+        its bin (:func:`gauge_bin_edges`): the value itself below 64, within 1/16 above.  ``p_at_least`` (``[G, T]``,
+        ``None`` without ``at_least``) is the fraction of the contributing replicas whose value is ``>= at_least``;
+        exact, as ``at_least`` must be a bin edge.  NaN where no replica contributes the tick."""
+        if self.dist_hist is None:
+            msg = "no distribution bands: run the sweep with SweepRunner(bands=..., dist_series=[...])"
+            raise ValueError(msg)
+        want = (str(getattr(key, "value", key)), entity_id)
+        if want not in self.dist_series:
+            msg = f"{want} is not among the sweep's distribution series {self.dist_series}"
+            raise KeyError(msg)
+        h = self.dist_hist[:, self.dist_series.index(want)]            # [G, T, n_bins]
+        G, T, B = h.shape
+        edges = gauge_bin_edges(B + 1)
+        p_idx = None
+        if at_least is not None:
+            p_idx = int(np.searchsorted(edges, at_least))
+            if p_idx > B or edges[min(p_idx, B)] != at_least:
+                lo, hi = int(edges[max(p_idx - 1, 0)]), (int(edges[p_idx]) if p_idx <= B else None)
+                msg = (f"at_least={at_least!r} is not a bin edge: p_at_least is exact at edges only; the neighbouring "
+                       f"edges are {lo} and {hi}" if hi is not None else
+                       f"at_least={at_least!r} is above the last bin edge {int(edges[B])}")
+                raise ValueError(msg)
+        cum = np.cumsum(h, axis=-1, dtype=np.int64)
+        n = cum[..., -1] if B else np.zeros((G, T), dtype=np.int64)
+        ok = n > 0
+        val = edges[:B].astype(np.float64)
+
+        def at_rank(r: np.ndarray) -> np.ndarray:     # the value of 0-based order statistic r: the first bin with cum > r
+            b = np.minimum((cum <= r[..., None]).sum(axis=-1), max(B - 1, 0))
+            return np.where(ok, val[b], np.nan)
+
+        nf = n.astype(np.float64)
+        qs = []
+        for qq in np.atleast_1d(np.asarray(q, dtype=np.float64)):
+            idx = nf * qq - 1.0                          # numpy's inverted_cdf: virtual index n q - 1, up to the next
+            prev = np.floor(idx)                         # order statistic unless it is whole
+            r = np.where(idx - prev == 0, prev, prev + 1)
+            qs.append(at_rank(np.clip(r, 0, np.maximum(nf - 1, 0)).astype(np.int64)))
+        first = np.where(ok, val[np.minimum((cum == 0).sum(axis=-1), max(B - 1, 0))], np.nan)
+        last = at_rank(np.maximum(n - 1, 0))
+        with np.errstate(invalid="ignore", divide="ignore"):
+            p = None if p_idx is None else np.where(ok, (n - (cum[..., p_idx - 1] if p_idx else 0)) / nf, np.nan)
+        return {"t": np.arange(T) * self.flat.sample_period, "n": n, "min": first, "max": last,
+                "q": np.stack(qs, axis=1) if qs else np.zeros((G, 0, T)), "p_at_least": p}
 
     def group_latency(self) -> dict[str, Any]:
         """Per group and window, over the group's replicas, the latency and throughput of the completions that
@@ -436,4 +525,12 @@ class SweepResults:
             out.lat_sum_lo = np.sum([p.lat_sum_lo for p in parts], axis=0, dtype=np.uint64)
         if all(p.group_size is not None for p in parts):
             out.group_size = np.sum([p.group_size for p in parts], axis=0, dtype=np.int64)
+        if all(p.dist_hist is not None for p in parts):       # counts over disjoint replicas: u32 sums, exact below 2^32
+            for p in parts:
+                if list(p.dist_series) != list(f.dist_series):
+                    msg = f"concatenate: distribution bands of different series ({f.dist_series} and {p.dist_series})"
+                    raise ValueError(msg)
+            out.dist_series = list(f.dist_series)
+            B = max(p.dist_hist.shape[-1] for p in parts)        # shards may size their bins differently: pad
+            out.dist_hist = np.sum([pad_dist_bins(p.dist_hist, B) for p in parts], axis=0, dtype=np.uint32)
         return out

@@ -38,7 +38,7 @@
 extern "C" {
 #endif
 
-#define AF_ABI_VERSION 5
+#define AF_ABI_VERSION 6
 
 typedef enum AfStatus {
     AF_OK = 0,
@@ -301,6 +301,29 @@ int af_bands_configure(af_engine* e, const AfBandOptions* opt);
  * capacity_windows), capacity_windows windows per group; *n_windows = the run's window count.  Any array may be NULL. */
 int af_fetch_latency_bands(af_engine* e, uint64_t* hist, uint64_t* sum_hi, uint64_t* sum_lo,
                            uint64_t capacity_windows, uint64_t* n_windows);
+
+/* Per-tick distribution bands of selected sampled series over the groups of af_bands_upload, accumulated on the device.
+ * series[0 .. n) are af_fetch_sampled indices (n_dist = n of them); NULL or n = 0 turns the distribution bands off
+ * (the default).  Every later af_run with groups then counts, for every group g, selected series s, tick k < n_ticks
+ * and value bin b < n_bins:
+ *   out[g][s][k][b]   replicas of g that contribute tick k with a value of series[s] in bin b
+ * Bins: a value v < 64 has bin v; above, 16 log-linear bins per octave, b = 64 + 16 (msb(v) - 6) + ((v >> (msb(v) - 4))
+ * & 15) with msb(v) the index of v's highest set bit, so a bin is at most 1/16 of its lower edge wide.  n_bins =
+ * bin(bound) + 1 for the bound of af_bands_upload's check (the request capacity or the largest ram_mb, swept values
+ * included, of the rows this engine was given); larger values cannot occur and would count in the last bin.  The bin
+ * edges do not depend on the launch, only their count does: shards of one sweep may differ in n_bins, and summing
+ * them takes padding the narrower ones with empty bins.  A replica contributes every tick it took
+ * before a stop flag ended it, with its value at that tick (0 included); a replica the thread-per-replica pass flags and
+ * the warp-per-replica pass re-runs inside the same af_run contributes once, in full; host-side re-runs add nothing.
+ * The counts are exact: a group holds fewer than 2^32 replicas.  Every other output is the same with distribution
+ * bands on or off.  Rejected (AF_ERR_INVALID, with a message) when a series is out of range, not sampled by the
+ * scenario or listed twice, when the scenario takes 5e7 ticks or more, or when the rows, (n_groups + 1) x n_dist x
+ * (n_ticks + 1) x n_bins x 4 bytes, exceed the device's memory; af_bands_upload and af_run check all of it again.
+ * AF_ERR_STATE before af_scenario_upload. */
+int af_dist_bands_configure(af_engine* e, const int32_t* series, int32_t n);
+/* distribution bands of the last af_run: out[g][s][k][b] for k < min(*n_ticks, capacity_ticks), capacity_ticks tick
+ * rows of *n_bins bins per (g, s); *n_ticks = the run's tick count, *n_bins its bins.  out = NULL: the sizes only. */
+int af_fetch_dist_bands(af_engine* e, uint32_t* out, uint64_t capacity_ticks, uint64_t* n_ticks, uint32_t* n_bins);
 
 /* AF-RNG known-answer hook: the device's random numbers outside the state machine, n values per call
  * (the streams of oracle/afrng.py; tests/test_gpu_rng.py compares them bit for bit with oracle/afrng_c):
