@@ -237,11 +237,15 @@ __global__ void af_selftest_rng_kernel(uint64_t seed, uint64_t replica, int kind
     }
 }
 
-// value of order statistic `rank` given the bin that holds it
-__device__ __forceinline__ double af_bin_value(int bin, uint64_t rank, uint64_t cum_before, uint32_t cnt) {
+// value of order statistic `rank` given the bin that holds it.  The two end bins also hold every latency the histogram
+// clamps into them, so they reach out to the replica's exact extremes (afh::hist_order_stat).
+__device__ __forceinline__ double af_bin_value(int bin, uint64_t rank, uint64_t cum_before, uint32_t cnt,
+                                               double lat_min, double lat_max) {
     const long long base = (long long)((1023 + AF_HIST_MIN_EXP) << AF_HIST_SUB_BITS);
     double lo = __longlong_as_double(((long long)bin + base) << (52 - AF_HIST_SUB_BITS));
     double hi = __longlong_as_double(((long long)bin + 1 + base) << (52 - AF_HIST_SUB_BITS));
+    if (bin == 0 && lat_min < lo) lo = lat_min;
+    if (bin == AF_HIST_BINS - 1 && lat_max > hi) hi = lat_max;
     double frac = ((double)(rank - cum_before) + 0.5) / (double)cnt;
     return lo + frac * (hi - lo);
 }
@@ -253,6 +257,7 @@ __global__ void af_percentile_kernel(const uint32_t* __restrict__ hist, AfReplic
     if (warp >= n_replicas) return;
     const uint32_t* row = hist + warp * AF_HIST_BINS;
     const uint64_t n = stats[warp].completed;
+    const double lat_min = stats[warp].lat_min, lat_max = stats[warp].lat_max;
     // target order statistics (numpy linear interpolation between two neighbours)
     const double qs[3] = {50.0, 95.0, 99.0};
     uint64_t rank[6]; double frac[3]; double val[6];
@@ -277,7 +282,7 @@ __global__ void af_percentile_kernel(const uint32_t* __restrict__ hist, AfReplic
         uint64_t before = carry + (incl - c);
 #pragma unroll
         for (int i = 0; i < 6; ++i)
-            if (c && rank[i] >= before && rank[i] < before + c) val[i] = af_bin_value(base + lane, rank[i], before, c);
+            if (c && rank[i] >= before && rank[i] < before + c) val[i] = af_bin_value(base + lane, rank[i], before, c, lat_min, lat_max);
         carry += __shfl_sync(0xFFFFFFFFu, incl, 31);
     }
     // each target was found by exactly one lane: sum-reduce to share it

@@ -237,13 +237,17 @@ inline double hist_bin_edge(int32_t idx) {
     double x; memcpy(&x, &bits, 8); return x;
 }
 
-// value of the order statistic `rank` (0-based) read off the histogram
-inline double hist_order_stat(const uint32_t* hist, uint64_t rank) {
+// value of the order statistic `rank` (0-based) read off the histogram.  The end bins also hold the latencies the
+// histogram clamps into them: bin 0 spans [min(edge(0), lat_min), edge(1)), the last bin [edge(B-1), max(edge(B),
+// lat_max)], lat_min / lat_max being the replica's exact extremes
+inline double hist_order_stat(const uint32_t* hist, uint64_t rank, double lat_min, double lat_max) {
     uint64_t cum = 0;
     for (int32_t b = 0; b < AF_HIST_BINS; ++b) {
         uint64_t c = hist[b];
         if (c && rank < cum + c) {
             double lo = hist_bin_edge(b), hi = hist_bin_edge(b + 1);
+            if (b == 0 && lat_min < lo) lo = lat_min;
+            if (b == AF_HIST_BINS - 1 && lat_max > hi) hi = lat_max;
             double frac = ((double)(rank - cum) + 0.5) / (double)c;
             return lo + frac * (hi - lo);
         }
@@ -252,15 +256,16 @@ inline double hist_order_stat(const uint32_t* hist, uint64_t rank) {
     return NAN;
 }
 
-// numpy.percentile(..., method="linear") evaluated on the histogram
-inline double hist_percentile(const uint32_t* hist, uint64_t n, double q) {
+// numpy.percentile(..., method="linear") evaluated on the histogram of a replica whose latencies span [lat_min, lat_max].
+// Without the extremes (a histogram summed over replicas has none) every bin keeps its own edges.
+inline double hist_percentile(const uint32_t* hist, uint64_t n, double q, double lat_min = INFINITY, double lat_max = 0.0) {
     if (n == 0) return NAN;
     double pos = q / 100.0 * (double)(n - 1);
     uint64_t lo = (uint64_t)floor(pos);
     double frac = pos - (double)lo;
-    double a = hist_order_stat(hist, lo);
+    double a = hist_order_stat(hist, lo, lat_min, lat_max);
     if (frac == 0.0 || lo + 1 >= n) return a;
-    double b = hist_order_stat(hist, lo + 1);
+    double b = hist_order_stat(hist, lo + 1, lat_min, lat_max);
     return a + frac * (b - a);
 }
 

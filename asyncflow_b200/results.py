@@ -34,14 +34,22 @@ EDGE_SERIES = "edge_concurrent_connection"
 LATENCY_ORDER = ("total_requests", "mean", "median", "std_dev", "p95", "p99", "min", "max")
 
 
-def hist_percentiles(hist: np.ndarray, q: float) -> np.ndarray:
+def hist_percentiles(hist: np.ndarray, q: float, *, lo: np.ndarray | None = None,
+                     hi: np.ndarray | None = None) -> np.ndarray:
     """numpy-'linear' percentile ``q`` of the completions each latency histogram counts (``hist[..., AF_HIST_BINS]``,
     the log-linear bins of the engine): the two order statistics around ``q / 100 * (n - 1)``, each placed inside its
     bin by its rank among the bin's counts, interpolated linearly.  NaN where a histogram is empty.  Returns
-    ``hist.shape[:-1]``."""
+    ``hist.shape[:-1]``.
+
+    ``lo`` / ``hi`` (``hist.shape[:-1]``): each histogram's exact smallest and largest latency (a replica's ``lat_min``
+    / ``lat_max``).  The end bins also count the latencies clamped into them, so with these given bin 0 spans
+    ``[min(edge(0), lo), edge(1))`` and the last bin ``[edge(B - 1), max(edge(B), hi)]`` -- the engine's per-replica
+    ``p50`` / ``p95`` / ``p99``.  Without them every bin keeps its own edges (histograms summed over replicas)."""
     h = np.asarray(hist)
     flat = h.reshape(-1, h.shape[-1])
     out = np.full(flat.shape[0], np.nan)
+    lat_lo = np.full(flat.shape[0], np.inf) if lo is None else np.asarray(lo, dtype=np.float64).reshape(-1)
+    lat_hi = np.zeros(flat.shape[0]) if hi is None else np.asarray(hi, dtype=np.float64).reshape(-1)
     base = (1023 + K.AF_HIST_MIN_EXP) << K.AF_HIST_SUB_BITS
     for c in range(0, flat.shape[0], 1024):                   # bounded temporaries: [rows, bins] at a time
         cum = np.cumsum(flat[c:c + 1024], axis=1, dtype=np.int64)
@@ -51,13 +59,16 @@ def hist_percentiles(hist: np.ndarray, q: float) -> np.ndarray:
             continue
         cum, n = cum[ok], n[ok]
         rows = flat[c:c + 1024][ok]
+        r_lo, r_hi = lat_lo[c:c + 1024][ok], lat_hi[c:c + 1024][ok]
 
-        def order_stat(rank: np.ndarray, cum=cum, rows=rows) -> np.ndarray:
+        def order_stat(rank: np.ndarray, cum=cum, rows=rows, r_lo=r_lo, r_hi=r_hi) -> np.ndarray:
             b = (cum <= rank[:, None]).sum(axis=1)          # searchsorted(cum, rank, side="right") per row
             b = np.minimum(b, cum.shape[1] - 1)
             before = np.where(b > 0, cum[np.arange(b.size), np.maximum(b - 1, 0)], 0)
             lo = ((b + base).astype(np.uint64) << np.uint64(52 - K.AF_HIST_SUB_BITS)).view(np.float64)
             hi = ((b + 1 + base).astype(np.uint64) << np.uint64(52 - K.AF_HIST_SUB_BITS)).view(np.float64)
+            lo = np.where((b == 0) & (r_lo < lo), r_lo, lo)
+            hi = np.where((b == cum.shape[1] - 1) & (r_hi > hi), r_hi, hi)
             frac = ((rank - before).astype(np.float64) + 0.5) / rows[np.arange(b.size), b].astype(np.float64)
             return lo + frac * (hi - lo)
 

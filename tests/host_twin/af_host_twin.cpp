@@ -21,8 +21,8 @@ extern "C" const char* af_twin_error() { return g_err.c_str(); }
 
 extern "C" int af_twin_trace_tick_capacity(const AfScenario* sc) { return afh::trace_tick_capacity(*sc); }
 
-extern "C" double af_twin_hist_percentile(const uint32_t* hist, uint64_t n, double q) {
-    return afh::hist_percentile(hist, n, q);
+extern "C" double af_twin_hist_percentile(const uint32_t* hist, uint64_t n, double q, double lat_min, double lat_max) {
+    return afh::hist_percentile(hist, n, q, lat_min, lat_max);
 }
 
 extern "C" int af_twin_run(const AfScenario* sc, const AfSweep* sw, uint64_t sweep_first, const AfOptions* opt,
@@ -56,9 +56,9 @@ extern "C" int af_twin_run(const AfScenario* sc, const AfSweep* sw, uint64_t swe
         afc::bind(W, base, 0);
         afc::run_replica(W, r);
         if (L.collect_hist && stats) {
-            stats[r].p50 = afh::hist_percentile(hist + r * AF_HIST_BINS, stats[r].completed, 50.0);
-            stats[r].p95 = afh::hist_percentile(hist + r * AF_HIST_BINS, stats[r].completed, 95.0);
-            stats[r].p99 = afh::hist_percentile(hist + r * AF_HIST_BINS, stats[r].completed, 99.0);
+            stats[r].p50 = afh::hist_percentile(hist + r * AF_HIST_BINS, stats[r].completed, 50.0, stats[r].lat_min, stats[r].lat_max);
+            stats[r].p95 = afh::hist_percentile(hist + r * AF_HIST_BINS, stats[r].completed, 95.0, stats[r].lat_min, stats[r].lat_max);
+            stats[r].p99 = afh::hist_percentile(hist + r * AF_HIST_BINS, stats[r].completed, 99.0, stats[r].lat_min, stats[r].lat_max);
         }
     }
     return AF_OK;
@@ -102,9 +102,9 @@ extern "C" int af_twin_run_lane(const AfScenario* sc, const AfSweep* sw, uint64_
     afl::run_lane(m, [&]() -> uint64_t { return next < n ? next++ : ~0ull; }, [](bool alive) { return alive; });
     if (C.collect_hist && stats)
         for (uint64_t r = 0; r < n; ++r) {
-            stats[r].p50 = afh::hist_percentile(hist + r * AF_HIST_BINS, stats[r].completed, 50.0);
-            stats[r].p95 = afh::hist_percentile(hist + r * AF_HIST_BINS, stats[r].completed, 95.0);
-            stats[r].p99 = afh::hist_percentile(hist + r * AF_HIST_BINS, stats[r].completed, 99.0);
+            stats[r].p50 = afh::hist_percentile(hist + r * AF_HIST_BINS, stats[r].completed, 50.0, stats[r].lat_min, stats[r].lat_max);
+            stats[r].p95 = afh::hist_percentile(hist + r * AF_HIST_BINS, stats[r].completed, 95.0, stats[r].lat_min, stats[r].lat_max);
+            stats[r].p99 = afh::hist_percentile(hist + r * AF_HIST_BINS, stats[r].completed, 99.0, stats[r].lat_min, stats[r].lat_max);
         }
     return AF_OK;
 }

@@ -74,9 +74,9 @@ extern "C" int af_split_twin_run_lane(const AfScenario* sc, const AfSweep* sw, u
     afl::run_lane(m, [&]() -> uint64_t { return next < n ? next++ : ~0ull; }, [](bool alive) { return alive; });
     if (C.collect_hist && stats)
         for (uint64_t r = 0; r < n; ++r) {
-            stats[r].p50 = afh::hist_percentile(hist + r * AF_HIST_BINS, stats[r].completed, 50.0);
-            stats[r].p95 = afh::hist_percentile(hist + r * AF_HIST_BINS, stats[r].completed, 95.0);
-            stats[r].p99 = afh::hist_percentile(hist + r * AF_HIST_BINS, stats[r].completed, 99.0);
+            stats[r].p50 = afh::hist_percentile(hist + r * AF_HIST_BINS, stats[r].completed, 50.0, stats[r].lat_min, stats[r].lat_max);
+            stats[r].p95 = afh::hist_percentile(hist + r * AF_HIST_BINS, stats[r].completed, 95.0, stats[r].lat_min, stats[r].lat_max);
+            stats[r].p99 = afh::hist_percentile(hist + r * AF_HIST_BINS, stats[r].completed, 99.0, stats[r].lat_min, stats[r].lat_max);
         }
     return AF_OK;
 }

@@ -122,7 +122,7 @@ def test_histogram_percentile_matches_numpy_within_two_percent():
     idx = (bits >> np.uint64(52 - K.AF_HIST_SUB_BITS)).astype(np.int64) - ((1023 + K.AF_HIST_MIN_EXP) << K.AF_HIST_SUB_BITS)
     hist = np.bincount(np.clip(idx, 0, K.AF_HIST_BINS - 1), minlength=K.AF_HIST_BINS).astype(np.uint32)
     for q in (50.0, 95.0, 99.0):
-        got = twin.lib().af_twin_hist_percentile(hist.ctypes.data, len(lat), q)
+        got = twin.lib().af_twin_hist_percentile(hist.ctypes.data, len(lat), q, lat.min(), lat.max())
         exact = float(np.percentile(lat, q))
         assert abs(got - exact) < 0.01 * exact
 

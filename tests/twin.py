@@ -43,7 +43,7 @@ def lib() -> C.CDLL:
         L = C.CDLL(str(build()))
         L.af_twin_error.restype = C.c_char_p
         L.af_twin_hist_percentile.restype = C.c_double
-        L.af_twin_hist_percentile.argtypes = [C.c_void_p, C.c_uint64, C.c_double]
+        L.af_twin_hist_percentile.argtypes = [C.c_void_p, C.c_uint64, C.c_double, C.c_double, C.c_double]
         L.af_twin_trace_tick_capacity.argtypes = [C.POINTER(K.AfScenario)]
         L.af_twin_run.argtypes = [
             C.POINTER(K.AfScenario), C.POINTER(K.AfSweep), C.c_uint64, C.POINTER(K.AfOptions),
