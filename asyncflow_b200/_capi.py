@@ -11,7 +11,7 @@ from __future__ import annotations
 import ctypes as C
 from pathlib import Path
 
-AF_ABI_VERSION = 6
+AF_ABI_VERSION = 7
 AF_HIST_BINS = 4096
 AF_HIST_SUB_BITS = 7
 AF_HIST_MIN_EXP = -20
@@ -125,6 +125,10 @@ class AfBandOptions(C.Structure):
     _fields_ = [("sampled", C.c_int32), ("latency_window_s", C.c_int32)]
 
 
+class AfOccupancyOptions(C.Structure):
+    _fields_ = [("on", C.c_int32), ("frac_bits", C.c_int32)]
+
+
 class EngineUnavailable(RuntimeError):
     """The CUDA engine cannot run here (library not built or no usable GPU)."""
 
@@ -138,7 +142,7 @@ EXPORTS = [
     "af_fetch_histograms", "af_fetch_throughput", "af_fetch_sampled", "af_fetch_trace_clocks",
     "af_fetch_trace_series", "af_reduce_histograms", "af_engine_set_mode", "af_last_run_passes",
     "af_selftest_rng", "af_bands_upload", "af_fetch_bands", "af_bands_configure", "af_fetch_latency_bands",
-    "af_dist_bands_configure", "af_fetch_dist_bands",
+    "af_dist_bands_configure", "af_fetch_dist_bands", "af_occupancy_configure", "af_fetch_occupancy",
 ]
 
 _lib = None
@@ -188,6 +192,8 @@ def load() -> C.CDLL:
     lib.af_fetch_latency_bands.argtypes = [vp, vp, vp, vp, u64, C.POINTER(u64)]
     lib.af_dist_bands_configure.argtypes = [vp, vp, C.c_int32]
     lib.af_fetch_dist_bands.argtypes = [vp, vp, u64, C.POINTER(u64), C.POINTER(C.c_uint32)]
+    lib.af_occupancy_configure.argtypes = [vp, C.POINTER(AfOccupancyOptions)]
+    lib.af_fetch_occupancy.argtypes = [vp, vp, u64, C.POINTER(C.c_int32)]
     for name in EXPORTS:
         fn = getattr(lib, name)
         if fn.restype is C.c_int and name not in ("af_abi_version",):

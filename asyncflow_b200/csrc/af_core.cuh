@@ -185,6 +185,8 @@ struct State {
     uint32_t* dist; const int32_t* dist_slot;
     uint64_t dist_series_words;
     uint32_t dist_bins, dist_pad;
+    // occupancy integrals: the replica's output row (nullptr: off; afl::occ_add, DESIGN.md §3.8), 2^f
+    uint64_t* occ; double occ_scale;
 };
 
 // Everything the kernel needs to know about sizes; built on the host.
@@ -223,6 +225,8 @@ struct BandArgs {
     uint32_t* dist_rows; const int32_t* dist_slot;
     uint64_t dist_group_words, dist_series_words;
     uint32_t dist_bins, dist_pad;
+    // occupancy integrals (occ == nullptr: off): [n_replicas][5 n_servers + n_edges] u64, occ_scale = 2^f
+    uint64_t* occ; double occ_scale;
 };
 
 constexpr int32_t NQ_CAP = 128;   // now-queue capacity (power of two)
@@ -327,6 +331,15 @@ static inline void w_sync() {}
 static inline void red_add_u32(uint32_t* p, uint32_t v) { *p += v; }
 static inline void red_add_u64(uint64_t* p, uint64_t v) { *p += v; }
 #endif
+
+// occupancy integrals (afl::occ_add): a count of requests in some state changes by delta at W.now -- lane 0 adds
+// delta * fixed(H - now) to the column of the replica's row (every lane runs this code)
+enum : int32_t { OC_RAM_WAIT = 0, OC_CPU_WAIT, OC_CPU, OC_IO, OC_RAM_MB, OC_WORDS };
+AF_IN void occ_add(const State& W, int32_t col, int32_t delta) {
+    if (W.occ != nullptr && lane_id() == 0)
+        red_add_u64(W.occ + col, (uint64_t)(int64_t)delta * afr::occ_fixed(W.horizon - W.now, W.occ_scale));
+}
+AF_IN void occ_srv(const State& W, uint32_t sidx, int32_t state, int32_t delta) { occ_add(W, OC_WORDS * (int32_t)sidx + state, delta); }
 
 // ---------------------------------------------------------------------------------
 // storage tiers: low slot numbers live in shared memory, the rest in the warp's HBM
@@ -583,6 +596,7 @@ AF_FN void edge_send(State& W, uint32_t slot, uint32_t e, uint32_t rid, uint32_t
         return;
     }
     E.conn += 1;
+    occ_add(W, OC_WORDS * AF_L.n_servers + (int32_t)e, 1);
     double effective = d.transit + E.spike;        // spike read at SEND time (edge.py:94-106)
     push_seq(W, W.now + effective, mk_payload(K_DELIVER, e, slot), s);
 }
@@ -617,6 +631,7 @@ AF_FN bool cpu_walk(State& W, ServerS& S, uint32_t sidx, uint32_t watch) {
     while (S.cpuq_head != NIL && S.cpu_free > 0) {
         uint32_t w = fifo_pop(W, S.cpuq_head, S.cpuq_tail);
         S.cpu_free -= 1;
+        occ_srv(W, sidx, OC_CPU, 1);
         hit = hit || w == watch;
         nq_push(W, I_CPU_OK, sidx, w);
     }
@@ -630,6 +645,7 @@ AF_FN void ram_walk(State& W, ServerS& S, uint32_t sidx) {
         const uint32_t need = S.ramq_head_need;      // kept beside the queue: no trip to the waiter's record
         if ((int32_t)need > S.ram_free) break;
         uint32_t w = fifo_pop(W, S.ramq_head, S.ramq_tail);
+        occ_srv(W, sidx, OC_RAM_WAIT, -1);
         if (S.ramq_head != NIL) S.ramq_head_need = tbl_endpoint(W)[pk_ep(rq_load(W, S.ramq_head).pack)].total_ram;
         S.ram_free -= (int32_t)need;
         nq_push(W, I_RAM_OK, sidx, w);
@@ -639,6 +655,7 @@ AF_FN void ram_walk(State& W, ServerS& S, uint32_t sidx) {
 AF_IN void ram_enqueue(State& W, ServerS& S, uint32_t sidx, uint32_t slot, uint32_t total_ram) {
     if (S.ramq_head == NIL) S.ramq_head_need = total_ram;
     fifo_push(W, S.ramq_head, S.ramq_tail, slot);
+    occ_srv(W, sidx, OC_RAM_WAIT, 1);
     ram_walk(W, S, sidx);
 }
 
@@ -655,14 +672,15 @@ AF_FN void run_steps(State& W, uint32_t slot, uint32_t sidx, uint32_t rid, uint3
         if (st < ep.n_steps) {
             const StepS sp = tbl_step(W)[ep.step_begin + st];
             if (sp.kind == AF_STEP_CPU) {
-                if (pack & PK_IO) { pack &= ~PK_IO; S.io_q -= 1; }
+                if (pack & PK_IO) { pack &= ~PK_IO; S.io_q -= 1; occ_srv(W, sidx, OC_IO, -1); }
                 if (!(pack & PK_CORE)) {             // cpu_req = CPU.get(1); yield cpu_req
                     if (S.cpuq_head == NIL && S.cpu_free > 0 && can_fuse(W)) {
                         S.cpu_free -= 1;             // granted, and its get event would run next
+                        occ_srv(W, sidx, OC_CPU, 1);
                         pack |= PK_CORE;
                     } else {
                         fifo_push(W, S.cpuq_head, S.cpuq_tail, slot);
-                        if (!cpu_walk(W, S, sidx, slot)) { pack |= PK_WAIT; S.ready_q += 1; }   // not cpu_req.triggered
+                        if (!cpu_walk(W, S, sidx, slot)) { pack |= PK_WAIT; S.ready_q += 1; occ_srv(W, sidx, OC_CPU_WAIT, 1); }   // not cpu_req.triggered
                         rq_set_pack(W, slot, pack);
                         return;
                     }
@@ -673,12 +691,13 @@ AF_FN void run_steps(State& W, uint32_t slot, uint32_t sidx, uint32_t rid, uint3
             }
             if (pack & PK_CORE) {                    // yield CPU.put(1): level rises NOW
                 S.cpu_free += 1;
+                occ_srv(W, sidx, OC_CPU, -1);
                 if (can_fuse(W)) { if (AF_UNLIKELY(S.cpuq_head != NIL)) cpu_walk(W, S, sidx, NIL); pack &= ~PK_CORE; continue; }
                 rq_set_pack(W, slot, pack);
                 nq_push(W, I_CPU_PUT, sidx, slot);
                 return;
             }
-            if (!(pack & PK_IO)) { pack |= PK_IO; S.io_q += 1; }
+            if (!(pack & PK_IO)) { pack |= PK_IO; S.io_q += 1; occ_srv(W, sidx, OC_IO, 1); }
             rq_set_pack(W, slot, pack);
             push(W, W.now + sp.dur, mk_payload(K_STEP_END, sidx, slot));
             return;
@@ -686,15 +705,17 @@ AF_FN void run_steps(State& W, uint32_t slot, uint32_t sidx, uint32_t rid, uint3
         // end of the endpoint (server.py:257-276)
         if (pack & PK_CORE) {                        // yield CPU.put(1)
             S.cpu_free += 1;
+            occ_srv(W, sidx, OC_CPU, -1);
             if (can_fuse(W)) { if (AF_UNLIKELY(S.cpuq_head != NIL)) cpu_walk(W, S, sidx, NIL); pack &= ~PK_CORE; continue; }
             rq_set_pack(W, slot, pack);
             nq_push(W, I_CPU_PUT, sidx, slot);
             return;
         }
-        if (pack & PK_IO) { pack &= ~PK_IO; S.io_q -= 1; }
+        if (pack & PK_IO) { pack &= ~PK_IO; S.io_q -= 1; occ_srv(W, sidx, OC_IO, -1); }
         rq_set_pack(W, slot, pack);
         if (ep.total_ram) {                          // yield RAM.put(total_ram): level rises NOW
             S.ram_in_use -= (int32_t)ep.total_ram;
+            occ_srv(W, sidx, OC_RAM_MB, -(int32_t)ep.total_ram);
             S.ram_free += (int32_t)ep.total_ram;
             if (!can_fuse(W)) { nq_push(W, I_RAM_PUT, sidx, slot); return; }
             if (AF_UNLIKELY(S.ramq_head != NIL)) ram_walk(W, S, sidx);   // the put event would run next: waiters, then forward
@@ -736,6 +757,7 @@ AF_IN void server_got(State& W, uint32_t slot, uint32_t sidx, const ReqRec& r) {
         }
         S.ram_free -= (int32_t)total_ram;            // granted, and its get event would run next
         S.ram_in_use += (int32_t)total_ram;
+        occ_srv(W, sidx, OC_RAM_MB, (int32_t)total_ram);
     }
     run_steps(W, slot, sidx, r.rid, pack);
 }
@@ -849,11 +871,12 @@ AF_IN void run_item(State& W, uint32_t item) {
         ServerS& S = tbl_server(W)[aux];
         ReqRec r = rq_load(W, slot);
         S.ram_in_use += (int32_t)tbl_endpoint(W)[pk_ep(r.pack)].total_ram;
+        occ_srv(W, aux, OC_RAM_MB, (int32_t)tbl_endpoint(W)[pk_ep(r.pack)].total_ram);
         run_steps(W, slot, aux, r.rid, r.pack);
     } else if (kind == I_CPU_OK) {                   // the CPU get event is processed
         ServerS& S = tbl_server(W)[aux];
         ReqRec r = rq_load(W, slot);
-        if (r.pack & PK_WAIT) { r.pack &= ~PK_WAIT; S.ready_q -= 1; }
+        if (r.pack & PK_WAIT) { r.pack &= ~PK_WAIT; S.ready_q -= 1; occ_srv(W, aux, OC_CPU_WAIT, -1); }
         run_steps(W, slot, aux, r.rid, r.pack | PK_CORE);
     } else if (kind == I_CPU_PUT) {
         on_cpu_put(W, slot, aux);
@@ -872,6 +895,7 @@ AF_IN void run_item(State& W, uint32_t item) {
 AF_IN void on_deliver(State& W, uint32_t slot, uint32_t e) {
     EdgeS& E = tbl_edge(W)[e];
     E.conn -= 1;
+    occ_add(W, OC_WORDS * AF_L.n_servers + (int32_t)e, -1);
     const uint32_t meta = E.meta;
     ReqRec r = rq_load(W, slot);
     r.pack += 1;                                     // record_hop(edge)
@@ -1197,6 +1221,12 @@ AF_IN void run_replica(State& W, uint64_t local_index, const BandArgs& band) {
     W.band = nullptr; W.band_from = 0; W.band_stride = band.stride; W.band_prev_off = (uint32_t)band.prev_off;
     W.lat = nullptr; W.lat_from = 0; W.lat_window = band.lat_window;
     W.dist = nullptr; W.dist_slot = band.dist_slot; W.dist_series_words = band.dist_series_words; W.dist_bins = band.dist_bins;
+    W.occ = nullptr; W.occ_scale = band.occ_scale;
+    if (band.occ != nullptr) {                        // a re-run starts over: the first pass's row is overwritten
+        const int32_t cols = OC_WORDS * AF_L.n_servers + AF_L.n_edges;
+        W.occ = band.occ + local_index * (uint64_t)cols;
+        for (int32_t c = lane_id(); c < cols; c += WARP) W.occ[c] = 0;
+    }
     if (band.stride || band.lat_window || band.dist_rows) {
         const uint64_t i = W.replica - band.first;
         const uint32_t g = i < band.n ? band.group[i] : band.groups;

@@ -92,10 +92,11 @@ __global__ void AF_LAUNCH_BOUNDS af_sim_kernel(const afc::BandArgs band) {
 // the band options ask for); <false, false> is the kernel without them.  kLean: the loop without spikes, outages,
 // traces, the general edge sampler and the endpoint draw (af_run picks it when aflh::lean_launch says the launch can
 // reach none of them).  kDist: the per-tick distribution bands of the selected series too (af_dist_bands_configure).
+// kOcc: the occupancy integrals too (af_occupancy_configure).
 #ifndef AF_LANE_MAX_THREADS
 #define AF_LANE_MAX_THREADS 384
 #endif
-template <bool kSampled = false, bool kLatency = false, bool kLean = false, bool kDist = false>
+template <bool kSampled = false, bool kLatency = false, bool kLean = false, bool kDist = false, bool kOcc = false>
 __global__ void __launch_bounds__(AF_LANE_MAX_THREADS, 1) af_lane_kernel() {
     const afl::Cfg& C = afl::c_cfg;
     const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
@@ -108,7 +109,7 @@ __global__ void __launch_bounds__(AF_LANE_MAX_THREADS, 1) af_lane_kernel() {
     m.g128 = gs + lane * 16u;
     m.g64 = gs + (size_t)C.gn128 * afl::STRIDE128 + lane * 8u;
     m.g32 = gs + (size_t)C.gn128 * afl::STRIDE128 + (size_t)C.gn64 * afl::STRIDE64 + lane * 4u;
-    afl::run_lane<kSampled, kLatency, kLean, kDist>(m,
+    afl::run_lane<kSampled, kLatency, kLean, kDist, kOcc>(m,
         [&]() -> uint64_t {
             const unsigned long long k = atomicAdd(C.work_counter, 1ull);
             return k < C.n_replicas ? (uint64_t)C.order[k] : ~0ull;
@@ -411,6 +412,10 @@ struct af_engine {
     DevBuf d_dist_slot, d_dist;
     bool last_dist = false; uint32_t last_dist_groups = 0, last_dist_ticks = 0, last_dist_bins = 0, last_dist_n = 0;
     uint64_t last_dist_series_words = 0;
+    // af_occupancy_configure: on / off and f; the [n][occ_cols] rows of the last run
+    AfOccupancyOptions occ_opt{0, 32};
+    DevBuf d_occ;
+    bool last_occ = false; int32_t last_occ_bits = 0, last_occ_cols = 0;
 
     int fail(int code, const std::string& m) { err = m; return code; }
     int cuda_fail(cudaError_t e, const char* what) {
@@ -426,6 +431,15 @@ static int upload_vec(af_engine* e, DevBuf& d, const std::vector<T>& h, const ch
     AF_CUDA(e, d.ensure(h.size() * sizeof(T)), what);
     if (!h.empty()) AF_CUDA(e, cudaMemcpyAsync(d.p, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice, e->stream), what);
     return AF_OK;
+}
+
+// the instantiation of af_lane_kernel for a launch's bands, build and occupancy
+template <bool S, bool L, bool Lean, bool D>
+static void (*lane_kernel_for(bool occ))() { return occ ? af_lane_kernel<S, L, Lean, D, true> : af_lane_kernel<S, L, Lean, D, false>; }
+template <bool S, bool L>
+static void (*lane_kernel_for(bool lean, bool dist, bool occ))() {
+    return lean ? (dist ? lane_kernel_for<S, L, true, true>(occ) : lane_kernel_for<S, L, true, false>(occ))
+                : (dist ? lane_kernel_for<S, L, false, true>(occ) : lane_kernel_for<S, L, false, false>(occ));
 }
 
 extern "C" {
@@ -485,7 +499,7 @@ void af_engine_destroy(af_engine* e) {
                       &e->d_tclk, &e->d_tser, &e->d_tcnt, &e->d_counter, &e->d_htot,
                       &e->d_okey, &e->d_oidx, &e->d_order, &e->d_okey64, &e->d_sort_tmp,
                       &e->d_band_group, &e->d_band, &e->d_band_from, &e->d_lat, &e->d_lat_from,
-                      &e->d_dist_slot, &e->d_dist};
+                      &e->d_dist_slot, &e->d_dist, &e->d_occ};
     for (DevBuf* b : bufs) b->release();
     cudaEventDestroy(e->ev_begin); cudaEventDestroy(e->ev_sim); cudaEventDestroy(e->ev_end);
     cudaStreamDestroy(e->stream);
@@ -681,6 +695,17 @@ int af_dist_bands_configure(af_engine* e, const int32_t* series, int32_t n) {
     return rc;
 }
 
+int af_occupancy_configure(af_engine* e, const AfOccupancyOptions* opt) {
+    if (!e || !opt) return AF_ERR_INVALID;
+    if (opt->on && (opt->frac_bits < 8 || opt->frac_bits > 32)) {
+        char b[160]; snprintf(b, sizeof b, "occupancy: %d fraction bits; 8 to 32 are supported", opt->frac_bits);
+        return e->fail(AF_ERR_INVALID, b);
+    }
+    e->occ_opt = *opt;
+    e->occ_opt.on = opt->on != 0;
+    return AF_OK;
+}
+
 int af_bands_configure(af_engine* e, const AfBandOptions* opt) {
     if (!e || !opt) return AF_ERR_INVALID;
     if (opt->latency_window_s != 0) {
@@ -845,6 +870,14 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
     if (lat && (rc = lat_check(e, e->band_groups))) return rc;
     const uint64_t lat_windows = lat ? afh::lat_windows(L.horizon_s, e->lat_window) : 0;
     const uint64_t lat_words = lat ? ((uint64_t)e->band_groups + 1) * lat_windows * afr::LAT_ROW : 0;
+    // ---- occupancy integrals: n x occ_cols u64 ----------------------------------------------------------------------
+    const bool occ = e->occ_opt.on != 0;
+    const int32_t occ_cols = afh::occ_cols(e->sc);
+    if (occ) {
+        std::string why;
+        if (!afh::occ_fits(e->sc, e->opt, e->band_swept_ram, e->band_swept_server, e->occ_opt.frac_bits, why))
+            return e->fail(AF_ERR_INVALID, why);
+    }
 
     // ---- launch shapes -------------------------------------------------------------------------------------
     // warp-per-replica: persistent CTAs of <= 4 warps (__launch_bounds__(128, AF_MIN_BLOCKS)), as many per SM as fit
@@ -870,15 +903,8 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
     // the lean build of the loop when the launch cannot reach what it leaves out; ASYNCFLOW_B200_LANE_FULL (A/B
     // experiments) keeps the full one
     const bool lean = lane && aflh::lean_launch(e->sc, o.trace_replicas) && getenv("ASYNCFLOW_B200_LANE_FULL") == nullptr;
-    void (*lane_kernel)() = lean ? (bands ? (lat ? af_lane_kernel<true, true, true> : af_lane_kernel<true, false, true>)
-                                          : (lat ? af_lane_kernel<false, true, true> : af_lane_kernel<false, false, true>))
-                                 : (bands ? (lat ? af_lane_kernel<true, true> : af_lane_kernel<true, false>)
-                                          : (lat ? af_lane_kernel<false, true> : af_lane_kernel<false, false>));
-    if (dist)
-        lane_kernel = lean ? (bands ? (lat ? af_lane_kernel<true, true, true, true> : af_lane_kernel<true, false, true, true>)
-                                    : (lat ? af_lane_kernel<false, true, true, true> : af_lane_kernel<false, false, true, true>))
-                           : (bands ? (lat ? af_lane_kernel<true, true, false, true> : af_lane_kernel<true, false, false, true>)
-                                    : (lat ? af_lane_kernel<false, true, false, true> : af_lane_kernel<false, false, false, true>));
+    void (*const lane_kernel)() = bands ? (lat ? lane_kernel_for<true, true>(lean, dist, occ) : lane_kernel_for<true, false>(lean, dist, occ))
+                                        : (lat ? lane_kernel_for<false, true>(lean, dist, occ) : lane_kernel_for<false, false>(lean, dist, occ));
     if (lane) {
         lsmem = (size_t)lane_warps * (size_t)C.warp_bytes;
         AF_CUDA(e, cudaFuncSetAttribute(lane_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lsmem), "smem attribute");
@@ -895,6 +921,7 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
         AF_CUDA(e, e->d_sp_rq.ensure(warp_slots * rq_sp * 16 + 16), "spill requests");
         AF_CUDA(e, e->d_sp_nx.ensure(warp_slots * rq_sp * 4 + 4), "spill requests");
     }
+    if (lane && occ) aflh::add_occupancy(C, 32, occ_cols, e->occ_opt.frac_bits);
     if (lane) {
         AF_CUDA(e, e->d_gtier.ensure(lgrid * (uint64_t)lane_warps * C.gwarp_bytes + 256), "lane global tiers");
         if ((rc = upload_vec(e, e->d_l_edges, e->lt.edges, "lane tables"))) return rc;
@@ -934,6 +961,7 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
         AF_CUDA(e, e->d_lat.ensure(lat_words * 8), "latency band rows");
         AF_CUDA(e, e->d_lat_from.ensure(n * 4), "latency band completions");
     }
+    if (occ) AF_CUDA(e, e->d_occ.ensure(n * (uint64_t)occ_cols * 8), "occupancy rows");
     // pull order: the first pass runs `workers` replicas at once (lanes, or warps without the thread-per-replica pass)
     const uint64_t workers = lane ? lgrid * (uint64_t)lane_warps * 32ull : warp_slots;
     const uint64_t wave = workers < n ? workers : n;
@@ -976,6 +1004,7 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
     G.redo_list = redo ? (const uint32_t*)e->d_redo_list.p : nullptr;
     G.redo_count = redo ? (const uint32_t*)e->d_redo_count.p : nullptr;
     G.seed = seed; G.replica_begin = begin; G.n_replicas = n;
+    if (occ) { band.occ = (uint64_t*)e->d_occ.p; band.occ_scale = ldexp(1.0, e->occ_opt.frac_bits); }
     if (bands || lat || dist) { band.group = (const uint32_t*)e->d_band_group.p; band.first = e->band_first; band.n = e->h_band_group.size(); band.groups = e->band_groups; }
     if (dist) {
         band.from = (const uint32_t*)e->d_band_from.p;
@@ -1019,6 +1048,7 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
             C.lat_rows = band.lat_rows; C.lat_from = (uint32_t*)e->d_lat_from.p;
             C.lat_window = e->lat_window; C.lat_windows = (int32_t)lat_windows;
         }
+        C.occ = band.occ;
     }
 
     // ---- enqueue ---------------------------------------------------------------------------------------------------
@@ -1100,6 +1130,7 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
     e->last_lat = lat; e->last_lat_groups = e->band_groups; e->last_lat_windows = lat_windows;
     e->last_dist = dist; e->last_dist_groups = e->band_groups; e->last_dist_ticks = dist_ticks; e->last_dist_bins = dist_bins;
     e->last_dist_n = (uint32_t)dist_n; e->last_dist_series_words = dist_series_words;
+    e->last_occ = occ; e->last_occ_bits = e->occ_opt.frac_bits; e->last_occ_cols = occ_cols;
     return AF_OK;
 }
 
@@ -1310,6 +1341,13 @@ int af_fetch_dist_bands(af_engine* e, uint32_t* out, uint64_t cap_ticks, uint64_
     AF_CUDA(e, cudaMemcpy2DAsync(out, cap_ticks * B * 4, e->d_dist.p, e->last_dist_series_words * 4, k * B * 4, rows,
                                  cudaMemcpyDeviceToHost, e->stream), "distribution bands D2H");
     return af_sync(e);
+}
+
+int af_fetch_occupancy(af_engine* e, uint64_t* out, uint64_t n, int32_t* frac_bits) {
+    if (!e) return AF_ERR_INVALID;
+    if (e->ran && !e->last_occ) return e->fail(AF_ERR_STATE, "the last run collected no occupancy (af_occupancy_configure)");
+    if (frac_bits) *frac_bits = e->last_occ_bits;
+    return fetch(e, out, e->d_occ, n * (uint64_t)e->last_occ_cols * 8, n, "occupancy D2H");
 }
 
 int af_fetch_trace_series(af_engine* e, uint64_t local, uint32_t* out, uint64_t cap_ticks, uint64_t* n_ticks) {

@@ -211,6 +211,38 @@ inline bool dist_bands_fit(const AfScenario& s, const AfOptions& o, uint64_t swe
     return false;
 }
 
+// Occupancy integrals (DESIGN.md §3.8): 5 columns per server (afl::OC_*), one per edge.
+inline int32_t occ_cols(const AfScenario& s) { return 5 * s.n_servers + s.n_edges; }
+// The most fraction bits f (at most 32) for which a column bounded by `bound` x `horizon_s` seconds stays below 2^64:
+// floor(log2((2^64 - 1) / (bound x horizon))); -1 when not even f = 0 fits.
+inline int32_t occ_frac_bits(uint64_t bound, int32_t horizon_s) {
+    const unsigned __int128 bh = (unsigned __int128)(bound ? bound : 1) * (uint64_t)(horizon_s > 0 ? horizon_s : 1);
+    if (bh > ~0ull) return -1;
+    const uint64_t q = ~0ull / (uint64_t)bh;
+    int32_t f = 63 - __builtin_clzll(q);
+    return f < 32 ? f : 32;
+}
+// The check af_occupancy_configure and af_run apply: 8 <= f <= 32, and bound x horizon x 2^f <= 2^64 - 1 for the
+// band_gauge_bound of the scenario, options and sweep (a count of requests is at most the request capacity, MB in use
+// at most the largest ram_mb).
+inline bool occ_fits(const AfScenario& s, const AfOptions& o, uint64_t swept_ram, int32_t swept_server, int32_t frac_bits,
+                     std::string& why) {
+    std::string what;
+    const uint64_t bound = band_gauge_bound(s, o, swept_ram, swept_server, what);
+    char b[400];
+    if (frac_bits < 8 || frac_bits > 32) {
+        snprintf(b, sizeof b, "occupancy: %d fraction bits; 8 to 32 are supported", frac_bits);
+        why = b;
+        return false;
+    }
+    if (((unsigned __int128)bound * (uint64_t)s.horizon_s << frac_bits) <= (unsigned __int128)~0ull) return true;
+    snprintf(b, sizeof b, "occupancy: a column of up to B = %llu (%s) x H = %d s in fixed point with f = %d fraction bits "
+             "could reach 2^64; this bound and horizon allow f <= %d", (unsigned long long)bound, what.c_str(), s.horizon_s,
+             frac_bits, occ_frac_bits(bound, s.horizon_s));
+    why = b;
+    return false;
+}
+
 inline void make_layout(const AfScenario& s, const AfOptions& o, int32_t n_sweep_cols, afc::Layout& L) {
     L.n_edges = s.n_edges; L.n_servers = s.n_servers; L.n_endpoints = s.n_endpoints; L.n_steps = s.n_steps;
     L.n_lb_edges = s.n_lb_edges; L.lb_algo = s.lb_algo; L.gen_edge = s.gen_edge; L.client_edge = s.client_edge;

@@ -187,6 +187,11 @@ struct Cfg {
     uint32_t* dist_rows; const int32_t* dist_slot;
     uint64_t dist_group_words, dist_series_words;
     int32_t dist_n, dist_bins;
+    // occupancy integrals (run_lane<*, *, *, *, true> only; DESIGN.md §3.8): occ_cols u64 accumulators per replica at
+    // elements gi_occ + col of the 64-bit global tier (RED during the run), written to occ[local * occ_cols + col] at
+    // write-back; occ_scale = 2^f (afr::occ_fixed)
+    uint64_t* occ; double occ_scale;
+    int32_t gi_occ, occ_cols;
 };
 
 
@@ -602,22 +607,34 @@ AFL_IN void gauge_touch(const St& W, const Mem& m, int32_t j, uint32_t v_old, in
         w32_st(m, dw, d | bit);
     }
 }
-template <bool kBands, bool kDist>
+// Occupancy integrals (kOcc; DESIGN.md §3.8): a count of requests in some state that changes by delta at W.now adds
+// delta * fixed(H - now) to its column, whatever the metrics mask samples -- the integral of the count over [0, H)
+// (u64 modular arithmetic: exact in any order, the sum below 2^64 by the choice of f).  Columns 5 s + OC_* of server s,
+// 5 n_servers + e of edge e.
+enum : int32_t { OC_RAM_WAIT = 0, OC_CPU_WAIT, OC_CPU, OC_IO, OC_RAM_MB, OC_WORDS };
+template <bool kOcc>
+AFL_IN void occ_add(const St& W, const Mem& m, int32_t col, int32_t delta) {
+    if constexpr (kOcc) red_add64(g64p(m, AFL_C.gi_occ + col), (uint64_t)(int64_t)delta * afr::occ_fixed(W.horizon - W.now, AFL_C.occ_scale));
+}
+AFL_IN int32_t occ_col(uint32_t sidx, int32_t state) { return OC_WORDS * (int32_t)sidx + state; }
+template <bool kBands, bool kDist, bool kOcc>
 AFL_IN void conn_add(const St& W, const Mem& m, uint32_t edge, int32_t delta) {
     const int32_t pw = AFL_C.o32_conn + (int32_t)edge;
     const uint32_t v = w32_ld(m, pw);
     if (AFL_C.metrics_mask & AF_METRIC_EDGE_CONN) gauge_touch<kBands, kDist>(W, m, 3 * AFL_C.n_servers + (int32_t)edge, v, delta);
+    occ_add<kOcc>(W, m, OC_WORDS * AFL_C.n_servers + (int32_t)edge, delta);
     w32_st(m, pw, v + (uint32_t)delta);
 }
 AFL_IN int32_t ib_word(uint32_t node, int32_t f) { return AFL_C.c_inbox + (int32_t)node * IB_WORDS + f; }      // cold
 AFL_IN int32_t sq_word(uint32_t sidx, int32_t f) { return AFL_C.c_srvq + (int32_t)sidx * SQ_WORDS + f; }       // cold
 AFL_IN int32_t sv_word(uint32_t sidx, int32_t f) { return AFL_C.o32_srv + (int32_t)sidx * SV_WORDS + f; }
 // field = SV_READY_Q / SV_IO_Q / SV_RAM_IN_USE (series 3 * sidx + 0 / 1 / 2)
-template <bool kBands, bool kDist>
+template <bool kBands, bool kDist, bool kOcc>
 AFL_IN void srv_gauge_add(const St& W, const Mem& m, uint32_t sidx, int32_t field, int32_t delta) {
     const int32_t pw = sv_word(sidx, field);
     const int32_t v = i32_ld(m, pw);
     if ((AFL_C.metrics_mask & 7u) == 7u) gauge_touch<kBands, kDist>(W, m, 3 * (int32_t)sidx + (field - SV_READY_Q), (uint32_t)v, delta);
+    occ_add<kOcc>(W, m, occ_col(sidx, field == SV_READY_Q ? OC_CPU_WAIT : (field == SV_IO_Q ? OC_IO : OC_RAM_MB)), delta);
     i32_st(m, pw, v + delta);
 }
 AFL_IN uint32_t gauge_value(const Mem& m, int32_t j) {
@@ -727,6 +744,18 @@ AFL_IN void dist_stop(const St& W, const Mem& m) {
     AFL_C.band_from[W.local] = n;
 }
 
+// ---- occupancy integrals: a replica starts with zeroed accumulators (a re-run of af_run's second pass starts over in
+//      the warp-per-replica engine) and writes them out with its other results
+AFL_IN void occ_start(const Mem& m) {
+#pragma unroll 1
+    for (int32_t c = 0; c < AFL_C.occ_cols; ++c) *g64p(m, AFL_C.gi_occ + c) = 0;
+}
+AFL_IN void occ_write(const St& W, const Mem& m) {
+#pragma unroll 1
+    for (int32_t c = 0; c < AFL_C.occ_cols; ++c)
+        AFL_C.occ[W.local * (uint64_t)AFL_C.occ_cols + (uint32_t)c] = ld_cg64(g64p(m, AFL_C.gi_occ + c));
+}
+
 // ---- Stores (mailboxes), Containers: as af_core.cuh ----------------------------------------------------
 // is the waiter FIFO whose head is cold word `head` empty?  (n_waiting == 0: all of them are, without looking)
 AFL_IN bool q_empty(const St& W, const Mem& m, int32_t head) { return AFL_LIKELY(W.n_waiting == 0) || c32_ld(m, head) == NIL; }
@@ -739,6 +768,7 @@ AFL_IN void consumer_get(St& W, const Mem& m, uint32_t node) {
 }
 // Container._trigger_get over the CPU queue: grant heads while a core is free
 // (returns true when `watch` was among the granted: its get is "triggered" at the call)
+template <bool kOcc>
 AFL_IN bool cpu_walk(St& W, const Mem& m, uint32_t sidx, uint32_t watch) {
     bool hit = false;
 #pragma unroll 1
@@ -746,12 +776,14 @@ AFL_IN bool cpu_walk(St& W, const Mem& m, uint32_t sidx, uint32_t watch) {
         const uint32_t w = fifo_pop(m, sq_word(sidx, SQ_CPUQ_HEAD), sq_word(sidx, SQ_CPUQ_TAIL));
         W.n_waiting -= 1;
         i32_st(m, sv_word(sidx, SV_CPU_FREE), i32_ld(m, sv_word(sidx, SV_CPU_FREE)) - 1);
+        occ_add<kOcc>(W, m, occ_col(sidx, OC_CPU), 1);
         hit = hit || w == watch;
         nq_push(W, m, I_CPU_OK, sidx, w);
     }
     return hit;
 }
 // ... over the RAM queue: grant heads while they fit, stop at the first that does not
+template <bool kOcc>
 AFL_IN void ram_walk(St& W, const Mem& m, uint32_t sidx) {
 #pragma unroll 1
     while (!q_empty(W, m, sq_word(sidx, SQ_RAMQ_HEAD))) {
@@ -759,6 +791,7 @@ AFL_IN void ram_walk(St& W, const Mem& m, uint32_t sidx) {
         if ((int32_t)need > i32_ld(m, sv_word(sidx, SV_RAM_FREE))) break;
         const uint32_t w = fifo_pop(m, sq_word(sidx, SQ_RAMQ_HEAD), sq_word(sidx, SQ_RAMQ_TAIL));
         W.n_waiting -= 1;
+        occ_add<kOcc>(W, m, occ_col(sidx, OC_RAM_WAIT), -1);
         const uint32_t h = c32_ld(m, sq_word(sidx, SQ_RAMQ_HEAD));
         if (h != NIL) c32_st(m, sq_word(sidx, SQ_RAMQ_NEED), ep_total_ram(m, pk_ep(rq_pack(W, m, h))));
         i32_st(m, sv_word(sidx, SV_RAM_FREE), i32_ld(m, sv_word(sidx, SV_RAM_FREE)) - (int32_t)need);
@@ -972,8 +1005,11 @@ enum : uint32_t { A_NONE = 0, A_NODE, A_STEPS, A_SEND, A_TIMER };
 // the same order with fewer instructions to fetch.  <S, L, false> compiles to the same code as before kLean existed.
 // `kDist`: the per-tick distribution bands of the selected series (Cfg.dist_*) too; <S, L, Lean, false> compiles to
 // the same code as before kDist existed.
+// `kOcc`: the occupancy integrals too (Cfg.occ*, occ_add); <S, L, Lean, D, false> compiles to the same code as before
+// kOcc existed.
 // ---------------------------------------------------------------------------------------------------
-template <bool kSampled = false, bool kLatency = false, bool kLean = false, bool kDist = false, class NextFn, class ConvFn>
+template <bool kSampled = false, bool kLatency = false, bool kLean = false, bool kDist = false, bool kOcc = false,
+          class NextFn, class ConvFn>
 AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
     const Cfg& C = AFL_C;
     St W;
@@ -991,6 +1027,7 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                 if constexpr (kSampled) band_start(W);
                 if constexpr (kLatency) lat_g = lat_group(W);
                 if constexpr (kDist) dist_start(W);
+                if constexpr (kOcc) occ_start(m);
                 // start order of the reference (simulation_runner.py:339-342, 301-336):
                 // spike timeline, outage timeline, generator, ..., collector
                 if (!kLean && C.n_spike > 0) {
@@ -1087,7 +1124,11 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
             const double tick = W.tick_time;
             if (tick < t_ev || (tick == t_ev && W.tick_seq < ev_seq)) take_ticks<kLean>(W, m, t_ev, ev_seq);
         }
-        if (AFL_UNLIKELY(finish)) { write_back<kLean>(W, m); active = false; }
+        if (AFL_UNLIKELY(finish)) {
+            write_back<kLean>(W, m);
+            if constexpr (kOcc) occ_write(W, m);
+            active = false;
+        }
         AFL_SYNC();
         if (is_event) { W.now = t_ev; W.n_events += 1; }
 
@@ -1105,7 +1146,7 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
         if (names_request) rq_load(W, m, slot, t0, rid, pack);
         if (is_event) {
             if (kind == K_DELIVER) {                          // edge.py:110-116: the edge's timeout fired
-                conn_add<kSampled, kDist>(W, m, aux, -1);
+                conn_add<kSampled, kDist, kOcc>(W, m, aux, -1);
                 const uint32_t meta = ro(C.edges + aux).meta;
                 pack += 1;                                     // record_hop(edge)
                 const uint32_t tk = (meta >> 3) & 3u;
@@ -1152,21 +1193,21 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                 consumer_get(W, m, NODE_CLIENT);
             } else if (kind == I_RAM_OK) {                     // the RAM get event is processed: the handler resumes
                 sidx = aux;
-                srv_gauge_add<kSampled, kDist>(W, m, sidx, SV_RAM_IN_USE, (int32_t)ep_total_ram(m, pk_ep(pack)));
+                srv_gauge_add<kSampled, kDist, kOcc>(W, m, sidx, SV_RAM_IN_USE, (int32_t)ep_total_ram(m, pk_ep(pack)));
                 act = A_STEPS;
             } else if (kind == I_CPU_OK) {                     // the CPU get event is processed
                 sidx = aux;
-                if (pack & PK_WAIT) { pack &= ~PK_WAIT; srv_gauge_add<kSampled, kDist>(W, m, sidx, SV_READY_Q, -1); }
+                if (pack & PK_WAIT) { pack &= ~PK_WAIT; srv_gauge_add<kSampled, kDist, kOcc>(W, m, sidx, SV_READY_Q, -1); }
                 pack |= PK_CORE;
                 act = A_STEPS;
             } else if (kind == I_CPU_PUT) {                    // waiters are re-examined, then the request goes on
                 sidx = aux;
-                cpu_walk(W, m, sidx, NIL);
+                cpu_walk<kOcc>(W, m, sidx, NIL);
                 pack &= ~PK_CORE;                              // core_locked = False; same step again
                 act = A_STEPS;
             } else {                                           // I_RAM_PUT: waiters first, then forward
                 sidx = aux;
-                ram_walk(W, m, sidx);
+                ram_walk<kOcc>(W, m, sidx);
                 edge = ro(C.servers + sidx).out_edge;
                 act = A_SEND;
             }
@@ -1199,11 +1240,12 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                         if (q_empty(W, m, sq_word(sidx, SQ_RAMQ_HEAD))) c32_st(m, sq_word(sidx, SQ_RAMQ_NEED), total_ram);
                         fifo_push(m, sq_word(sidx, SQ_RAMQ_HEAD), sq_word(sidx, SQ_RAMQ_TAIL), slot);
                         W.n_waiting += 1;
-                        ram_walk(W, m, sidx);
+                        occ_add<kOcc>(W, m, occ_col(sidx, OC_RAM_WAIT), 1);
+                        ram_walk<kOcc>(W, m, sidx);
                         go = false;
                     } else {
                         i32_st(m, sv_word(sidx, SV_RAM_FREE), i32_ld(m, sv_word(sidx, SV_RAM_FREE)) - (int32_t)total_ram);   // granted, and its get event would run next
-                        srv_gauge_add<kSampled, kDist>(W, m, sidx, SV_RAM_IN_USE, (int32_t)total_ram);
+                        srv_gauge_add<kSampled, kDist, kOcc>(W, m, sidx, SV_RAM_IN_USE, (int32_t)total_ram);
                     }
                 }
                 if (go) act = A_STEPS;
@@ -1258,30 +1300,32 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                 if (st < ep.n_steps) {
                     const StepP sp = ro(C.steps + ep.step_begin + st);
                     if (sp.kind == AF_STEP_CPU) {
-                        if (pack & PK_IO) { pack &= ~PK_IO; srv_gauge_add<kSampled, kDist>(W, m, sidx, SV_IO_Q, -1); }
+                        if (pack & PK_IO) { pack &= ~PK_IO; srv_gauge_add<kSampled, kDist, kOcc>(W, m, sidx, SV_IO_Q, -1); }
                         if (!(pack & PK_CORE)) {             // cpu_req = CPU.get(1); yield cpu_req
                             if (can_fuse(W) && i32_ld(m, sv_word(sidx, SV_CPU_FREE)) > 0 && q_empty(W, m, sq_word(sidx, SQ_CPUQ_HEAD))) {
                                 i32_st(m, sv_word(sidx, SV_CPU_FREE), i32_ld(m, sv_word(sidx, SV_CPU_FREE)) - 1);     // granted, and its get event would run next
+                                occ_add<kOcc>(W, m, occ_col(sidx, OC_CPU), 1);
                                 pack |= PK_CORE;
                             } else {
                                 fifo_push(m, sq_word(sidx, SQ_CPUQ_HEAD), sq_word(sidx, SQ_CPUQ_TAIL), slot);
                                 W.n_waiting += 1;
-                                if (!cpu_walk(W, m, sidx, slot)) { pack |= PK_WAIT; srv_gauge_add<kSampled, kDist>(W, m, sidx, SV_READY_Q, 1); }   // not cpu_req.triggered
+                                if (!cpu_walk<kOcc>(W, m, sidx, slot)) { pack |= PK_WAIT; srv_gauge_add<kSampled, kDist, kOcc>(W, m, sidx, SV_READY_Q, 1); }   // not cpu_req.triggered
                                 break;
                             }
                         }
                     } else {
                         if (pack & PK_CORE) {                // yield CPU.put(1): level rises NOW
                             i32_st(m, sv_word(sidx, SV_CPU_FREE), i32_ld(m, sv_word(sidx, SV_CPU_FREE)) + 1);
+                            occ_add<kOcc>(W, m, occ_col(sidx, OC_CPU), -1);
                             if (can_fuse(W)) {
-                                if (AFL_UNLIKELY(!q_empty(W, m, sq_word(sidx, SQ_CPUQ_HEAD)))) cpu_walk(W, m, sidx, NIL);
+                                if (AFL_UNLIKELY(!q_empty(W, m, sq_word(sidx, SQ_CPUQ_HEAD)))) cpu_walk<kOcc>(W, m, sidx, NIL);
                                 pack &= ~PK_CORE;
                                 continue;
                             }
                             nq_push(W, m, I_CPU_PUT, sidx, slot);
                             break;
                         }
-                        if (!(pack & PK_IO)) { pack |= PK_IO; srv_gauge_add<kSampled, kDist>(W, m, sidx, SV_IO_Q, 1); }
+                        if (!(pack & PK_IO)) { pack |= PK_IO; srv_gauge_add<kSampled, kDist, kOcc>(W, m, sidx, SV_IO_Q, 1); }
                     }
                     const double dur = sp.c_dur >= 0 ? row_val(m, sp.c_dur) : sp.dur;
                     tm_t = W.now + dur; tm_payload = mk_payload(K_STEP_END, sidx, slot); tm_seq = W.seq++;
@@ -1291,21 +1335,22 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                 // end of the endpoint (server.py:257-276)
                 if (pack & PK_CORE) {                        // yield CPU.put(1)
                     i32_st(m, sv_word(sidx, SV_CPU_FREE), i32_ld(m, sv_word(sidx, SV_CPU_FREE)) + 1);
+                    occ_add<kOcc>(W, m, occ_col(sidx, OC_CPU), -1);
                     if (can_fuse(W)) {
-                        if (AFL_UNLIKELY(!q_empty(W, m, sq_word(sidx, SQ_CPUQ_HEAD)))) cpu_walk(W, m, sidx, NIL);
+                        if (AFL_UNLIKELY(!q_empty(W, m, sq_word(sidx, SQ_CPUQ_HEAD)))) cpu_walk<kOcc>(W, m, sidx, NIL);
                         pack &= ~PK_CORE;
                         continue;
                     }
                     nq_push(W, m, I_CPU_PUT, sidx, slot);
                     break;
                 }
-                if (pack & PK_IO) { pack &= ~PK_IO; srv_gauge_add<kSampled, kDist>(W, m, sidx, SV_IO_Q, -1); }
+                if (pack & PK_IO) { pack &= ~PK_IO; srv_gauge_add<kSampled, kDist, kOcc>(W, m, sidx, SV_IO_Q, -1); }
                 const uint32_t total_ram = ep.c_ram >= 0 ? (uint32_t)row_val(m, ep.c_ram) : ep.total_ram;
                 if (total_ram) {                             // yield RAM.put(total_ram): level rises NOW
-                    srv_gauge_add<kSampled, kDist>(W, m, sidx, SV_RAM_IN_USE, -(int32_t)total_ram);
+                    srv_gauge_add<kSampled, kDist, kOcc>(W, m, sidx, SV_RAM_IN_USE, -(int32_t)total_ram);
                     i32_st(m, sv_word(sidx, SV_RAM_FREE), i32_ld(m, sv_word(sidx, SV_RAM_FREE)) + (int32_t)total_ram);
                     if (!can_fuse(W)) { nq_push(W, m, I_RAM_PUT, sidx, slot); break; }
-                    if (AFL_UNLIKELY(!q_empty(W, m, sq_word(sidx, SQ_RAMQ_HEAD)))) ram_walk(W, m, sidx);   // the put event would run next: waiters, then forward
+                    if (AFL_UNLIKELY(!q_empty(W, m, sq_word(sidx, SQ_RAMQ_HEAD)))) ram_walk<kOcc>(W, m, sidx);   // the put event would run next: waiters, then forward
                 }
                 edge = ro(C.servers + sidx).out_edge;
                 act = A_SEND;
@@ -1398,7 +1443,7 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                     rq_release(W, m, slot);
                 } else {
                     rq_pack_set(W, m, slot, pack);              // (the one store of the record on the request's way out of a node)
-                    conn_add<kSampled, kDist>(W, m, edge, 1);
+                    conn_add<kSampled, kDist, kOcc>(W, m, edge, 1);
                     double effective = transit;
                     if (!kLean && C.n_spike > 0) effective = transit + f64_ld(m, C.o64_spike + (int32_t)edge);   // spike read at SEND time (edge.py:94-106)
                     else effective = transit + 0.0;         // (-0.0 + 0.0 = +0.0, as with a spike table of zeros)

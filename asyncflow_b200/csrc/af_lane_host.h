@@ -280,4 +280,12 @@ inline bool make_cfg(const AfScenario& s, const AfOptions& o, const Tables& t, i
     return true;
 }
 
+// The occupancy integrals' accumulators (run_lane<*, *, *, *, true>): `cols` more elements of the 64-bit global tier,
+// right after the gauges' accumulators, and the scale 2^f (the caller sets C.occ, the [n][cols] output).
+inline void add_occupancy(afl::Cfg& C, int32_t lanes, int32_t cols, int32_t frac_bits) {
+    C.gi_occ = C.gn64; C.gn64 += cols; C.occ_cols = cols;
+    C.gwarp_bytes += (uint64_t)cols * 8 * (uint64_t)lanes;
+    C.occ_scale = ldexp(1.0, frac_bits);
+}
+
 }  // namespace aflh

@@ -122,6 +122,17 @@ AF_HD uint64_t lat_fixed32(double lat) {
 #endif
 }
 
+// Occupancy integrals (DESIGN.md §3.8): the time left to the horizon, rest = H - now >= 0, in fixed point with f fraction
+// bits, round-to-nearest-even(rest * 2^f), scale = 2^f (the scaling is exact).  A count that changes by delta at now adds
+// delta * occ_fixed(H - now) to its column: the column ends as the integral of the count over [0, H) in u64.
+AF_HD uint64_t occ_fixed(double rest, double scale) {
+#if defined(__CUDA_ARCH__)
+    return (uint64_t)__double2ull_rn(rest * scale);
+#else
+    return (uint64_t)nearbyint(rest * scale);
+#endif
+}
+
 // ln(x), finite normal x > 0 (fdlibm e_log.c scheme; see oracle/afrng.py:af_log)
 AF_HD_NOINLINE double af_log(double x) {
     const double ln2_hi = 6.93147180369123816490e-01, ln2_lo = 1.90821492927058770002e-10,

@@ -195,6 +195,21 @@ class Engine:
                     "af_dist_bands_configure")
         self._dist_n = int(s.size)
 
+    def configure_occupancy(self, on: bool = True, frac_bits: int = 32) -> None:
+        """Occupancy integrals from the next run on (:meth:`occupancy`): per replica, the request-seconds spent in each
+        state in fixed point with ``frac_bits`` fraction bits -- ``af_occupancy_configure``."""
+        opt = K.AfOccupancyOptions(int(bool(on)), int(frac_bits))
+        self._check(self._lib.af_occupancy_configure(self._h, C.byref(opt)), "af_occupancy_configure")
+
+    def occupancy(self, out: np.ndarray | None = None) -> tuple[np.ndarray, int]:
+        """Occupancy integrals of the last run: ``([n, 5 n_servers + n_edges] u64, f)`` -- the column layout of
+        ``af_fetch_occupancy``, ``value / 2**f`` request-seconds (MB-seconds for ``ram_mb``)."""
+        flat = self.flat
+        out = np.empty((self._n, 5 * flat.n_servers + flat.n_edges), dtype=np.uint64) if out is None else out
+        f = C.c_int32()
+        self._check(self._lib.af_fetch_occupancy(self._h, out.ctypes.data, self._n, C.byref(f)), "af_fetch_occupancy")
+        return out, int(f.value)
+
     def dist_bands(self) -> np.ndarray:
         """Distribution bands of the last run: ``[G, n_dist, T, n_bins]`` u32 -- per group, selected series, tick and
         value bin (``results.gauge_bin_edges``), the replicas that contribute the tick with a value in the bin

@@ -32,6 +32,12 @@ from .flatten import FlatScenario
 SERVER_SERIES = ("ready_queue_len", "event_loop_io_sleep", "ram_in_use")
 EDGE_SERIES = "edge_concurrent_connection"
 LATENCY_ORDER = ("total_requests", "mean", "median", "std_dev", "p95", "p99", "min", "max")
+#: the occupancy integrals' states of a server, in column order (``af_fetch_occupancy``); an edge's one state
+OCC_SERVER_STATES = ("ram_wait", "cpu_wait", "cpu", "io", "ram_mb")
+OCC_EDGE_STATE = "transit"
+#: the occupancy state whose count a sampled gauge reads
+GAUGE_STATE = {"ready_queue_len": "cpu_wait", "event_loop_io_sleep": "io", "ram_in_use": "ram_mb",
+               "edge_concurrent_connection": "transit"}
 
 
 def hist_percentiles(hist: np.ndarray, q: float, *, lo: np.ndarray | None = None,
@@ -106,6 +112,21 @@ def pad_dist_bins(hist: np.ndarray, n_bins: int) -> np.ndarray:
     out = np.zeros(hist.shape[:-1] + (int(n_bins),), dtype=hist.dtype)
     out[..., :b] = hist
     return out
+
+
+def occupancy_columns(flat: FlatScenario) -> list[tuple[str, str]]:
+    """``(entity_id, state)`` of each occupancy column: five per server (:data:`OCC_SERVER_STATES`), then one per edge."""
+    return ([(sid, st) for sid in flat.server_ids for st in OCC_SERVER_STATES]
+            + [(eid, OCC_EDGE_STATE) for eid in flat.edge_ids])
+
+
+def occ_frac_bits(bound: int, horizon_s: int) -> int:
+    """The most fraction bits f <= 32 with ``bound * horizon_s * 2**f <= 2**64 - 1`` (the engine's ``afh::occ_frac_bits``):
+    ``bound`` is the largest count a column can hold -- the request capacity or the largest ``ram_mb``."""
+    bh = max(int(bound), 1) * max(int(horizon_s), 1)
+    if bh > (1 << 64) - 1:
+        return -1
+    return min(32, (((1 << 64) - 1) // bh).bit_length() - 1)
 
 
 def series_index(flat: FlatScenario, key: Any, entity_id: str) -> int | None:
@@ -297,6 +318,10 @@ class SweepResults:
         # with a value in the bin -- [G, n_dist, T, n_bins] u32
         self.dist_series: list[tuple[str, str]] = []
         self.dist_hist: np.ndarray | None = None
+        # occupancy integrals (SweepRunner(occupancy=True)): per replica and column (occ_columns), the request-seconds
+        # in that state over [0, horizon) in fixed point with occ_frac_bits fraction bits -- [n, 5 n_servers + n_edges] u64
+        self.occupancy: np.ndarray | None = None
+        self.occ_frac_bits: int = 0
 
     def __len__(self) -> int:
         return int(self.stats.shape[0])
@@ -394,6 +419,7 @@ class SweepResults:
                                                                           self.lat_sum_hi, self.lat_sum_lo)
         out.group_size = self.group_size
         out.dist_series, out.dist_hist = self.dist_series, self.dist_hist
+        out.occupancy, out.occ_frac_bits = g(self.occupancy), self.occ_frac_bits
         return out
 
     def bands(self, key: Any, entity_id: str) -> dict[str, np.ndarray]:
@@ -485,6 +511,67 @@ class SweepResults:
         return {"t": np.arange(T) * self.flat.sample_period, "n": n, "min": first, "max": last,
                 "q": np.stack(qs, axis=1) if qs else np.zeros((G, 0, T)), "p_at_least": p}
 
+    @property
+    def occ_columns(self) -> list[tuple[str, str]]:
+        """``(entity_id, state)`` of each column of :attr:`occupancy`."""
+        return occupancy_columns(self.flat)
+
+    def _occ_column(self, state: str, entity_id: str) -> int:
+        if self.occupancy is None:
+            msg = "no occupancy: run the sweep with SweepRunner(occupancy=True)"
+            raise ValueError(msg)
+        try:
+            return self.occ_columns.index((entity_id, state))
+        except ValueError:
+            msg = f"no occupancy column ({entity_id!r}, {state!r}): states {OCC_SERVER_STATES} of a server, {OCC_EDGE_STATE!r} of an edge"
+            raise KeyError(msg) from None
+
+    def time_in(self, state: str, entity_id: str) -> np.ndarray:
+        """Per replica, the request-seconds spent in ``state`` at ``entity_id`` over the run, ``[n]`` float64: the
+        integral over [0, horizon) of the number of requests in that state (MB-seconds for ``"ram_mb"``).  A server's
+        states are ``ram_wait`` (blocked on RAM), ``cpu_wait`` (queued for a core), ``cpu`` (holding a core), ``io`` and
+        ``ram_mb``; an edge's is ``transit``."""
+        j = self._occ_column(state, entity_id)
+        return self.occupancy[:, j].astype(np.float64) * 2.0 ** -self.occ_frac_bits
+
+    def time_average(self, key: Any, entity_id: str) -> np.ndarray:
+        """Per replica, the exact time-weighted mean over [0, horizon) of a sampled gauge (``key`` / ``entity_id`` as
+        ``ResultsAnalyzer.get_series`` takes them), ``[n]`` float64.  :meth:`sampled_mean` reads the same gauge at the
+        collector's ticks only; this counts every change, however short, whether the scenario samples the gauge or not."""
+        name = str(getattr(key, "value", key))
+        if name not in GAUGE_STATE:
+            msg = f"unknown sampled metric {name!r}"
+            raise KeyError(msg)
+        return self.time_in(GAUGE_STATE[name], entity_id) / float(self.flat.horizon_s)
+
+    def breakdown(self, select: Any = None) -> dict[str, Any]:
+        """Where the selected replicas' requests spent their time (``select``: any numpy index of the rows, default all):
+        per occupancy column, ``{"entity", "state"}`` (lists), ``"raw"`` (the column summed exactly over the replicas,
+        Python ints in units of 2**-f s), ``"seconds"`` (float64), ``"share"`` (of the request-seconds of every column but
+        ``ram_mb``; NaN for ``ram_mb``, which counts MB-seconds) and ``"per_request"`` (seconds per generated request).
+        ``per_request`` is a finite-horizon Little's-law ratio: the time requests spend in a state over [0, horizon)
+        divided by the requests generated, so it includes the time of requests still in flight at the horizon."""
+        if self.occupancy is None:
+            msg = "no occupancy: run the sweep with SweepRunner(occupancy=True)"
+            raise ValueError(msg)
+        occ = self.occupancy if select is None else self.occupancy[select]
+        occ = occ.reshape(-1, occ.shape[-1])
+        hi = (occ >> np.uint64(32)).sum(axis=0, dtype=np.uint64)           # exact while fewer than 2^32 replicas
+        lo = (occ & np.uint64(0xFFFFFFFF)).sum(axis=0, dtype=np.uint64)
+        raw = [(int(h) << 32) + int(w) for h, w in zip(hi, lo)]
+        f = self.occ_frac_bits
+        seconds = np.array([r / (1 << f) for r in raw], dtype=np.float64)
+        cols = self.occ_columns
+        req = np.array([st != "ram_mb" for _, st in cols])
+        total = sum(r for r, q in zip(raw, req) if q) / (1 << f)
+        gen = self.stats["generated"] if select is None else self.stats["generated"][select]
+        n_gen = float(np.asarray(gen, dtype=np.float64).sum())
+        with np.errstate(invalid="ignore", divide="ignore"):
+            share = np.where(req, seconds / total if total > 0 else np.nan, np.nan)
+            per_request = seconds / n_gen if n_gen > 0 else np.full(len(cols), np.nan)
+        return {"entity": [e for e, _ in cols], "state": [st for _, st in cols], "raw": raw, "seconds": seconds,
+                "share": share, "per_request": per_request}
+
     def group_latency(self) -> dict[str, Any]:
         """Per group and window, over the group's replicas, the latency and throughput of the completions that
         finish in the window (``SweepRunner(latency_window_s=w)``): ``{"t", "n", "rps", "mean", "p50", "p95",
@@ -544,4 +631,10 @@ class SweepResults:
             out.dist_series = list(f.dist_series)
             B = max(p.dist_hist.shape[-1] for p in parts)        # shards may size their bins differently: pad
             out.dist_hist = np.sum([pad_dist_bins(p.dist_hist, B) for p in parts], axis=0, dtype=np.uint32)
+        if all(p.occupancy is not None for p in parts):       # per-replica rows: one scale for all of them
+            bits = sorted({p.occ_frac_bits for p in parts})
+            if len(bits) > 1:
+                msg = f"concatenate: occupancy rows in different fixed-point scales (fraction bits {bits})"
+                raise ValueError(msg)
+            out.occupancy, out.occ_frac_bits = np.concatenate([p.occupancy for p in parts]), bits[0]
         return out

@@ -38,7 +38,7 @@
 extern "C" {
 #endif
 
-#define AF_ABI_VERSION 6
+#define AF_ABI_VERSION 7
 
 typedef enum AfStatus {
     AF_OK = 0,
@@ -324,6 +324,32 @@ int af_dist_bands_configure(af_engine* e, const int32_t* series, int32_t n);
 /* distribution bands of the last af_run: out[g][s][k][b] for k < min(*n_ticks, capacity_ticks), capacity_ticks tick
  * rows of *n_bins bins per (g, s); *n_ticks = the run's tick count, *n_bins its bins.  out = NULL: the sizes only. */
 int af_fetch_dist_bands(af_engine* e, uint32_t* out, uint64_t capacity_ticks, uint64_t* n_ticks, uint32_t* n_bins);
+
+/* Occupancy integrals: per replica, the exact request-seconds spent in each state over [0, horizon), accumulated on the
+ * device.  C = 5 n_servers + n_edges u64 columns per replica:
+ *   5 s + 0  ram_wait  requests of server s blocked on its RAM (a RAM.get not granted at once)
+ *   5 s + 1  cpu_wait  requests in server s's ready queue (the sampled ready_queue_len)
+ *   5 s + 2  cpu       requests holding one of server s's cores (cpu_cores - free cores)
+ *   5 s + 3  io        requests in server s's I/O wait (the sampled event_loop_io_sleep)
+ *   5 s + 4  ram_mb    MB of server s's RAM reserved (the sampled ram_in_use): MB-seconds
+ *   5 n_servers + e    requests in transit on edge e (the sampled edge_concurrent_connection)
+ * A count n(t) that changes by d_i at times t_i < H (H = horizon_s) adds d_i x round-to-nearest-even((H - t_i) x 2^f)
+ * to its column in u64 modular arithmetic: the final value is the integral of n over [0, H) in fixed point with
+ * f = frac_bits fraction bits, within (changes / 2) x 2^-f of the exact integral, and the same bits in any summation
+ * order.  Every state change counts whatever the scenario samples.  A replica the thread-per-replica pass flags and
+ * the warp-per-replica pass re-runs inside the same af_run gets the re-run's row; a replica that stays stopped holds
+ * what it accumulated up to the stop.  Every other output is the same with occupancy on or off.
+ * on = 1 turns it on for every later af_run until changed.  af_run refuses (AF_ERR_INVALID, with a message) a launch
+ * whose bound B (the request capacity or the largest ram_mb, swept values included) does not fit B x H x 2^f <= 2^64 - 1;
+ * af_occupancy_configure refuses frac_bits outside [8, 32].  Pick f once for a whole sweep so that its shards share a
+ * scale. */
+typedef struct AfOccupancyOptions {
+    int32_t on;                 /* 0: off (default)                                                          */
+    int32_t frac_bits;          /* f, 8..32                                                                  */
+} AfOccupancyOptions;
+int af_occupancy_configure(af_engine* e, const AfOccupancyOptions* opt);
+/* occupancy of the last af_run: out[n][C] (C as above); *frac_bits = its f.  AF_ERR_STATE when it was off. */
+int af_fetch_occupancy(af_engine* e, uint64_t* out, uint64_t n, int32_t* frac_bits);
 
 /* AF-RNG known-answer hook: the device's random numbers outside the state machine, n values per call
  * (the streams of oracle/afrng.py; tests/test_gpu_rng.py compares them bit for bit with oracle/afrng_c):
