@@ -1,16 +1,17 @@
 """CPU tier: per-tick sampled-metric bands (af_bands_upload / af_fetch_bands).  Both state machines, driven with their
-difference rows by tests/host_twin/af_band_twin.cpp, must give per group and tick exactly the integer sums of the
+difference rows by the CPU twin (tests/twin.py), must give per group and tick exactly the integer sums of the
 oracle's sampled series over the group's replicas: first-hand, stitched (a replica the thread-per-replica pass stops
 and the warp-per-replica pass re-runs from its stop tick), truncated (a stopped replica that is not re-run), and with
 every other output unchanged by the bands."""
 
 from __future__ import annotations
 
-import band_twin as BT
+import band_ref
 import des_port
 import fuzz
 import numpy as np
 import pytest
+import twin
 from helpers import PARITY_CASES, SEED, load_scenario, oracle_series_matrix
 from twin_engine import TwinEngine
 
@@ -25,14 +26,14 @@ def oracle_matrix(payload, flat, replica: int) -> np.ndarray:
     """[n_series, T] series of one oracle replica (a series the scenario does not sample is 0)."""
     o = des_port.simulate(payload, seed=SEED, replica=replica)
     m = oracle_series_matrix(o, flat).astype(np.uint64)
-    T = BT.ticks(flat)
+    T = twin.ticks(flat)
     assert m.shape[1] in (0, T)
     return m if m.shape[1] == T else np.zeros((flat.n_series, T), dtype=np.uint64)
 
 
 def expected(flat, mats: list[np.ndarray], groups, n_groups: int, upto=None):
     """Per-group sums of the series matrices; replica i contributes ticks < upto[i] (default: all)."""
-    T, S = BT.ticks(flat), flat.n_series
+    T, S = twin.ticks(flat), flat.n_series
     cnt = np.zeros((n_groups, T), dtype=np.uint64)
     s = np.zeros((n_groups, S, T), dtype=np.uint64)
     sq = np.zeros((n_groups, S, T), dtype=np.uint64)
@@ -45,16 +46,16 @@ def expected(flat, mats: list[np.ndarray], groups, n_groups: int, upto=None):
 
 
 def assert_bands(flat, rows, n_groups, want):
-    got = BT.scan(flat, rows, n_groups)
+    got = band_ref.scan(flat, rows, n_groups)
     for name, a, b in zip(("count", "sum", "sumsq"), got, want):
         assert a.dtype == b.dtype and np.array_equal(a, b), name
 
 
 def test_band_twin_reports_the_kernels_tick_count():
     flat = flatten(load_scenario("c1_my_service.yml", 7))
-    assert abs(BT.ticks(flat) - 7 / flat.sample_period) <= 1
+    assert abs(twin.ticks(flat) - 7 / flat.sample_period) <= 1
     o = des_port.simulate(load_scenario("c1_my_service.yml", 7), seed=SEED, replica=0)
-    assert oracle_series_matrix(o, flat).shape[1] == BT.ticks(flat)
+    assert oracle_series_matrix(o, flat).shape[1] == twin.ticks(flat)
 
 
 @pytest.mark.parametrize("engine", ["lane", "warp"])
@@ -64,8 +65,8 @@ def test_bands_equal_the_oracle_sums(name, engine):
     flat = flatten(payload)
     n, begin = 4, 2
     groups = np.array([1, 0, 1, 0], dtype=np.uint32)
-    run = BT.run_lane if engine == "lane" else BT.run_warp
-    out = run(flat, seed=SEED, n=n, replica_begin=begin, groups=groups, n_groups=2, band_first=begin)
+    run = twin.run_lane if engine == "lane" else twin.run_warp
+    out = run(flat, seed=SEED, n=n, replica_begin=begin, groups=groups, n_groups=2, band_first=begin, sampled=True)
     assert (out["stats"]["flags"] & STOPS == 0).all()
     mats = [oracle_matrix(payload, flat, begin + i) for i in range(n)]
     want = expected(flat, mats, groups, 2)
@@ -82,16 +83,18 @@ def test_flagged_replicas_rerun_from_their_stop_tick_give_the_full_sums():
     payload, flat = _overloaded()
     n = 6
     groups = np.array([0, 1, 2, 0, 1, 2], dtype=np.uint32)
-    lane = BT.run_lane(flat, seed=SEED, n=n, groups=groups, n_groups=3, event_capacity=24, request_capacity=12, lane_bytes=520)
+    lane = twin.run_lane(flat, seed=SEED, n=n, groups=groups, n_groups=3, event_capacity=24, request_capacity=12, lane_bytes=520,
+                         sampled=True)
     flagged = np.flatnonzero(lane["stats"]["flags"] & REDO)
     assert flagged.size >= 1, "no replica stopped: the capacities do not force the second pass"
-    assert all(0 < int(lane["band_from"][i]) < BT.ticks(flat) for i in flagged)
-    out = BT.run_warp(flat, seed=SEED, n=n, groups=groups, n_groups=3, redo=flagged, band_from=lane["band_from"], into=lane)
+    assert all(0 < int(lane["band_from"][i]) < twin.ticks(flat) for i in flagged)
+    out = twin.run_warp(flat, seed=SEED, n=n, groups=groups, n_groups=3, redo=flagged, band_from=lane["band_from"], into=lane,
+                         sampled=True)
     assert (out["stats"]["flags"] & STOPS == 0).all()
     mats = [oracle_matrix(payload, flat, i) for i in range(n)]
     assert_bands(flat, out["band_rows"], 3, expected(flat, mats, groups, 3))
     # the stitched replicas' other outputs are the warp engine's first-hand ones
-    full = BT.run_warp(flat, seed=SEED, n=n, groups=groups, n_groups=3)
+    full = twin.run_warp(flat, seed=SEED, n=n, groups=groups, n_groups=3, sampled=True)
     for k in ("stats", "sent", "dropped", "samp_sum", "samp_max", "hist", "thr"):
         assert out[k].tobytes() == full[k].tobytes(), k
 
@@ -100,16 +103,17 @@ def test_a_stopped_replica_leaves_its_group_at_its_stop_tick():
     """Not re-run (LANE mode, or a flag the second pass does not take): the replica counts up to its stop tick, its sums
     are the oracle's truncated there, and the frozen ticks to the horizon add nothing."""
     payload, flat = _overloaded()
-    n, T = 6, BT.ticks(flat)
+    n, T = 6, twin.ticks(flat)
     groups = np.array([0, 0, 0, 1, 1, 1], dtype=np.uint32)
-    out = BT.run_lane(flat, seed=SEED, n=n, groups=groups, n_groups=2, event_capacity=24, request_capacity=12, lane_bytes=520)
+    out = twin.run_lane(flat, seed=SEED, n=n, groups=groups, n_groups=2, event_capacity=24, request_capacity=12, lane_bytes=520,
+                        sampled=True)
     stopped = (out["stats"]["flags"] & STOPS) != 0
     assert stopped.any() and (out["stats"]["n_ticks"] == T).all()      # (n_ticks counts the frozen ticks)
     upto = np.where(stopped, out["band_from"], T).astype(np.int64)
     assert (upto[stopped] < T).all()
     mats = [oracle_matrix(payload, flat, i) for i in range(n)]
     assert_bands(flat, out["band_rows"], 2, expected(flat, mats, groups, 2, upto))
-    cnt = BT.scan(flat, out["band_rows"], 2)[0]
+    cnt = band_ref.scan(flat, out["band_rows"], 2)[0]
     i = int(np.flatnonzero(stopped)[0])
     k, g = int(upto[i]), int(groups[i])
     assert cnt[g, k] < 3 and (cnt[g, :int(upto[groups == g].min())] == 3).all()
@@ -118,14 +122,14 @@ def test_a_stopped_replica_leaves_its_group_at_its_stop_tick():
 @pytest.mark.parametrize("engine", ["lane", "warp"])
 def test_bands_change_no_other_output(engine):
     payload, flat = _overloaded()
-    run = BT.run_lane if engine == "lane" else BT.run_warp
+    run = twin.run_lane if engine == "lane" else twin.run_warp
     kw = dict(seed=SEED, n=5, replica_begin=1, groups=np.array([0, 1, 0, 1, 0], dtype=np.uint32), n_groups=2,
               band_first=1, trace=3, clock_cap=5000, event_capacity=24, request_capacity=12)
     if engine == "lane":
         kw["lane_bytes"] = 520
-    on, off = run(flat, bands=True, **kw), run(flat, bands=False, **kw)
+    on, off = run(flat, sampled=True, **kw), run(flat, sampled=False, **kw)
     assert (on["stats"]["flags"] & STOPS).any()
-    for k in BT.OUTPUTS:
+    for k in twin.OUTPUTS:
         assert on[k].tobytes() == off[k].tobytes(), k
     assert not off["band_rows"].any() and on["band_rows"].any()
 
@@ -139,8 +143,8 @@ def test_fuzzed_scenarios_and_sweeps(seed):
     groups = np.array([0, 1, 1, 0], dtype=np.uint32)
     mats = [oracle_matrix(spec.payload_for(payload, i), flat, i) for i in range(n)]
     want = expected(flat, mats, groups, 2)
-    for run in (BT.run_lane, BT.run_warp):
-        out = run(flat, seed=SEED, n=n, sweep=spec, groups=groups, n_groups=2)
+    for run in (twin.run_lane, twin.run_warp):
+        out = run(flat, seed=SEED, n=n, sweep=spec, groups=groups, n_groups=2, sampled=True)
         assert (out["stats"]["flags"] & STOPS == 0).all()
         assert_bands(flat, out["band_rows"], 2, want)
 
@@ -149,21 +153,21 @@ def test_replicas_without_a_group_contribute_nothing():
     payload = load_scenario("c3_lb_two_servers.yml", 12)
     flat = flatten(payload)
     groups = np.array([0, 0], dtype=np.uint32)                 # replicas 1, 2 of 0..3
-    out = BT.run_lane(flat, seed=SEED, n=4, groups=groups, n_groups=1, band_first=1)
+    out = twin.run_lane(flat, seed=SEED, n=4, groups=groups, n_groups=1, band_first=1, sampled=True)
     mats = [oracle_matrix(payload, flat, r) for r in (1, 2)]
     assert_bands(flat, out["band_rows"], 1, expected(flat, mats, groups, 1))
 
 
 def test_sumsq_wrap_is_rejected_and_names_the_bound():
     flat = flatten(load_scenario("c1_my_service.yml", 5))
-    ok, bound, what = BT.sumsq_fits(flat, 1000, request_capacity=4096)
+    ok, bound, what = twin.sumsq_fits(flat, 1000, request_capacity=4096)
     assert ok and bound >= 4096
-    ok, bound, what = BT.sumsq_fits(flat, 1 << 40, request_capacity=(1 << 20) - 1)
+    ok, bound, what = twin.sumsq_fits(flat, 1 << 40, request_capacity=(1 << 20) - 1)
     assert not ok and bound == (1 << 20) - 1 and "request capacity" in what
     spec = SweepSpec(flat, 2, {("server_ram_mb", flat.server_ids[0]): [512.0, 2147483000.0]})
-    ok, bound, what = BT.sumsq_fits(flat, 5, request_capacity=1024, sweep=spec)
+    ok, bound, what = twin.sumsq_fits(flat, 5, request_capacity=1024, sweep=spec)
     assert not ok and bound == 2147483000 and "swept ram_mb" in what
-    assert BT.sumsq_fits(flat, 3, request_capacity=1024, sweep=spec)[0]
+    assert twin.sumsq_fits(flat, 3, request_capacity=1024, sweep=spec)[0]
 
 
 # ---- SweepRunner: groups are given per SWEEP ROW and follow the rows through the launch order ---------------------------
@@ -182,9 +186,9 @@ class BandTwinEngine(TwinEngine):
         self._bands = None
         if g is not None:
             ng = self.n_groups
-            out = BT.run_lane(self.flat, seed=seed, n=end - begin, replica_begin=begin, sweep=self.sweep, groups=g,
-                              n_groups=ng, band_first=self.band_first)
-            self._bands = BT.scan(self.flat, out["band_rows"], ng)
+            out = twin.run_lane(self.flat, seed=seed, n=end - begin, replica_begin=begin, sweep=self.sweep, groups=g,
+                                n_groups=ng, band_first=self.band_first, sampled=True)
+            self._bands = band_ref.scan(self.flat, out["band_rows"], ng)
 
     def bands(self):
         return self._bands
@@ -213,10 +217,10 @@ def test_sweep_runner_groups_rows_under_a_balanced_launch_order():
     for a, b in zip((res.band_count, res.band_sum, res.band_sumsq), want):
         assert np.array_equal(a, b)
     gb = res.group_bands("ready_queue_len", sw.flat.server_ids[0])
-    assert gb["mean"].shape == (3, BT.ticks(sw.flat)) and np.array_equal(gb["n"], want[0])
+    assert gb["mean"].shape == (3, twin.ticks(sw.flat)) and np.array_equal(gb["n"], want[0])
     s0 = want[1][:, 0, :].astype(np.float64)
     np.testing.assert_allclose(gb["mean"], s0 / 2)
-    assert np.allclose(gb["t"], np.arange(BT.ticks(sw.flat)) * sw.flat.sample_period)
+    assert np.allclose(gb["t"], np.arange(twin.ticks(sw.flat)) * sw.flat.sample_period)
 
 
 def test_sweep_runner_shard_maps_rows_through_replica_ids():
@@ -285,10 +289,10 @@ def test_a_horizon_with_more_ticks_than_the_band_rows_hold_is_refused():
     payload = load_scenario("c1_my_service.yml", 86_400)
     payload["sim_settings"]["sample_period_s"] = 0.001
     flat = flatten(payload)
-    assert BT.ticks(flat) == 50_000_000
-    ok, why = BT.ticks_fit(flat)
+    assert twin.ticks(flat) == 50_000_000
+    ok, why = twin.ticks_fit(flat)
     assert not ok and "86400" in why and "ticks or more" in why
     with pytest.raises(RuntimeError, match="ticks or more"):
-        BT.run_lane(flat, seed=SEED, n=1, groups=np.zeros(1, dtype=np.uint32), n_groups=1)
+        twin.run_lane(flat, seed=SEED, n=1, groups=np.zeros(1, dtype=np.uint32), n_groups=1, sampled=True)
     payload["sim_settings"]["total_simulation_time"] = 49_000                        # 4.9e7 ticks: they fit
-    assert BT.ticks_fit(flatten(payload))[0]
+    assert twin.ticks_fit(flatten(payload))[0]

@@ -1,5 +1,5 @@
 """CPU tier: per-tick distribution bands (af_dist_bands_configure / af_fetch_dist_bands).  Both state machines, driven
-with their difference rows by tests/host_twin/af_dist_twin.cpp, must give per group, tick and value bin exactly the
+with their difference rows by the CPU twin (tests/twin.py), must give per group, tick and value bin exactly the
 histogram of the oracle's sampled series over the group's replicas: first-hand, stitched (a replica the
 thread-per-replica pass stops and the warp-per-replica pass re-runs from its stop tick), truncated (a stopped replica
 that is not re-run, its zeros included), with every other output unchanged; and the host side must read quantiles,
@@ -7,11 +7,11 @@ extremes and exceedance off the counts as numpy reads them off the values."""
 
 from __future__ import annotations
 
-import band_twin as BT
+import band_ref
 import des_port
-import dist_twin as DT
 import numpy as np
 import pytest
+import twin
 from helpers import PARITY_CASES, SEED, load_scenario, oracle_series_matrix
 
 from asyncflow_b200 import flatten
@@ -29,7 +29,7 @@ def bins_of(values: np.ndarray, B: int) -> np.ndarray:
 def oracle_matrix(payload, flat, replica: int) -> np.ndarray:
     o = des_port.simulate(payload, seed=SEED, replica=replica)
     m = oracle_series_matrix(o, flat)
-    T = BT.ticks(flat)
+    T = twin.ticks(flat)
     return m if m.shape[1] == T else np.zeros((flat.n_series, T), dtype=np.uint32)
 
 
@@ -44,18 +44,18 @@ def expected(mats, series, groups, G: int, T: int, B: int, upto=None) -> np.ndar
 
 
 def got(out, G: int, T: int) -> np.ndarray:
-    return DT.scan(out["dist_rows"], G, T)
+    return band_ref.dist_scan(out["dist_rows"], G, T)
 
 
 def test_gauge_bin_mirror_matches_the_c_function():
-    B = DT.gauge_bin(0xFFFFFFFF) + 1
+    B = twin.gauge_bin(0xFFFFFFFF) + 1
     edges = gauge_bin_edges(B + 1)
     assert list(edges[:64]) == list(range(64)) and (np.diff(edges) > 0).all()
     assert (np.diff(edges)[64:] <= edges[64:-1] / 16).all()                   # at most 1/16 of the lower edge wide
     vals = np.unique(np.concatenate([np.arange(300), edges[:-1] - 1, edges[:-1], edges[:-1] + 1,
                                      np.random.default_rng(1).integers(0, 2 ** 32, 2000)]))
     vals = vals[(vals >= 0) & (vals < 2 ** 32)]
-    want = np.array([DT.gauge_bin(int(v)) for v in vals])
+    want = np.array([twin.gauge_bin(int(v)) for v in vals])
     np.testing.assert_array_equal(bins_of(vals, B), want)
 
 
@@ -67,10 +67,10 @@ def test_rows_equal_the_oracle_histogram(name, engine):
     n, begin = 4, 2
     groups = np.array([1, 0, 1, 0], dtype=np.uint32)
     series = [j for j in range(flat.n_series) if j % 2 == 0] or [0]
-    run = DT.run_lane if engine == "lane" else DT.run_warp
+    run = twin.run_lane if engine == "lane" else twin.run_warp
     out = run(flat, seed=SEED, n=n, replica_begin=begin, series=series, groups=groups, n_groups=2, band_first=begin)
     assert (out["stats"]["flags"] & STOPS == 0).all()
-    T, B = BT.ticks(flat), out["dist_rows"].shape[3]
+    T, B = twin.ticks(flat), out["dist_rows"].shape[3]
     mats = [oracle_matrix(payload, flat, begin + i) for i in range(n)]
     np.testing.assert_array_equal(got(out, 2, T), expected(mats, series, groups, 2, T, B))
 
@@ -85,21 +85,21 @@ def test_a_stitched_replica_counts_once_and_equals_the_oracle():
     n, series = 6, [0, 1, 2]
     groups = np.array([0, 1, 2, 0, 1, 2], dtype=np.uint32)
     kw = dict(seed=SEED, n=n, series=series, groups=groups, n_groups=3, bin_capacity=16384)
-    lane = DT.run_lane(flat, event_capacity=24, request_capacity=12, lane_bytes=520, **kw)
+    lane = twin.run_lane(flat, event_capacity=24, request_capacity=12, lane_bytes=520, **kw)
     flagged = np.flatnonzero(lane["stats"]["flags"] & STOPS)
-    assert flagged.size >= 1 and all(0 < int(lane["band_from"][i]) < BT.ticks(flat) for i in flagged)
-    out = DT.run_warp(flat, redo=flagged, into=lane, **kw)
-    T, B = BT.ticks(flat), out["dist_rows"].shape[3]
+    assert flagged.size >= 1 and all(0 < int(lane["band_from"][i]) < twin.ticks(flat) for i in flagged)
+    out = twin.run_warp(flat, redo=flagged, into=lane, **kw)
+    T, B = twin.ticks(flat), out["dist_rows"].shape[3]
     mats = [oracle_matrix(payload, flat, i) for i in range(n)]
     np.testing.assert_array_equal(got(out, 3, T), expected(mats, series, groups, 3, T, B))
 
 
 def test_a_truncated_replica_contributes_its_ticks_before_the_stop_zeros_included():
     payload, flat = _overloaded()
-    n, T = 6, BT.ticks(flat)
+    n, T = 6, twin.ticks(flat)
     series = [0, 1, 2]
     groups = np.array([0, 0, 0, 1, 1, 1], dtype=np.uint32)
-    out = DT.run_lane(flat, seed=SEED, n=n, series=series, groups=groups, n_groups=2, event_capacity=24,
+    out = twin.run_lane(flat, seed=SEED, n=n, series=series, groups=groups, n_groups=2, event_capacity=24,
                       request_capacity=12, lane_bytes=520)
     stopped = (out["stats"]["flags"] & STOPS) != 0
     assert stopped.any()
@@ -119,11 +119,11 @@ def test_cross_checks_with_the_sampled_bands():
     flat = flatten(payload)
     series = list(range(flat.n_series))
     groups = np.array([0, 1, 1, 0, 0], dtype=np.uint32)
-    for run in (DT.run_lane, DT.run_warp):
+    for run in (twin.run_lane, twin.run_warp):
         out = run(flat, seed=SEED, n=5, series=series, groups=groups, n_groups=2, sampled=True)
-        T = BT.ticks(flat)
+        T = twin.ticks(flat)
         d = got(out, 2, T)
-        cnt, s, _ = BT.scan(flat, out["band_rows"], 2)
+        cnt, s, _ = band_ref.scan(flat, out["band_rows"], 2)
         np.testing.assert_array_equal(d.sum(axis=3), np.repeat(cnt[:, None, :], len(series), axis=1))
         edges = gauge_bin_edges(d.shape[3]).astype(np.uint64)
         small = d[..., 64:].sum(axis=-1) == 0
@@ -140,16 +140,16 @@ def test_every_other_output_is_unchanged(sampled, window, lean):
               lean=lean)
     if not lean:
         kw.update(trace=3, clock_cap=5000)
-    on = DT.run_lane(flat, series=[0, 2], **kw)
-    off = DT.run_lane(flat, series=[], **kw)
+    on = twin.run_lane(flat, series=[0, 2], **kw)
+    off = twin.run_lane(flat, series=[], **kw)
     assert (on["stats"]["flags"] & STOPS).any() and on["dist_rows"].any()
-    for k in (*BT.OUTPUTS, "band_rows", "band_from", "lat_rows", "lat_from"):
+    for k in (*twin.OUTPUTS, "band_rows", "band_from", "lat_rows", "lat_from"):
         if k == "band_from" and not sampled:
             continue                                        # (written by the distribution bands alone when on)
         assert on[k].tobytes() == off[k].tobytes(), k
     wkw = {k: v for k, v in kw.items() if k not in ("lane_bytes", "lean")}
-    w_on, w_off = DT.run_warp(flat, series=[0, 2], **wkw), DT.run_warp(flat, series=[], **wkw)
-    for k in (*BT.OUTPUTS, "band_rows", "lat_rows"):
+    w_on, w_off = twin.run_warp(flat, series=[0, 2], **wkw), twin.run_warp(flat, series=[], **wkw)
+    for k in (*twin.OUTPUTS, "band_rows", "lat_rows"):
         assert w_on[k].tobytes() == w_off[k].tobytes(), k
 
 
@@ -157,25 +157,25 @@ def test_lean_and_full_builds_give_the_same_rows():
     payload = load_scenario("c3_lb_two_servers.yml", 30)
     flat = flatten(payload)
     kw = dict(seed=SEED, n=6, series=[0, 3, 4], groups=np.array([0, 1, 2, 0, 1, 2], dtype=np.uint32), n_groups=3)
-    a, b = DT.run_lane(flat, lean=True, **kw), DT.run_lane(flat, lean=False, **kw)
+    a, b = twin.run_lane(flat, lean=True, **kw), twin.run_lane(flat, lean=False, **kw)
     assert a["dist_rows"].tobytes() == b["dist_rows"].tobytes()
 
 
 def test_bad_series_and_oversized_rows_are_refused():
     flat = flatten(load_scenario("c3_lb_two_servers.yml", 30))
-    assert DT.fits(flat, [0, 3], 10)[0]
+    assert twin.dist_fits(flat, [0, 3], 10)[0]
     for bad, why in (([flat.n_series], "out of range"), ([-1], "out of range"), ([0, 0], "listed twice")):
-        ok, _, _, msg = DT.fits(flat, bad, 1)
+        ok, _, _, msg = twin.dist_fits(flat, bad, 1)
         assert not ok and "distribution bands" in msg and why in msg
-    ok, T, B, msg = DT.fits(flat, list(range(flat.n_series)), 100_000, mem_total=80 << 30, request_capacity=(1 << 20) - 1)
+    ok, T, B, msg = twin.dist_fits(flat, list(range(flat.n_series)), 100_000, mem_total=80 << 30, request_capacity=(1 << 20) - 1)
     assert not ok and "GB of rows" in msg and "request capacity" in msg
     payload = load_scenario("c1_my_service.yml", 86_400)
     payload["sim_settings"]["sample_period_s"] = 0.001
-    ok, _, _, msg = DT.fits(flatten(payload), [0], 1)
+    ok, _, _, msg = twin.dist_fits(flatten(payload), [0], 1)
     assert not ok and "ticks or more" in msg
     payload = load_scenario("c1_my_service.yml", 10)
     payload["sim_settings"]["enabled_sample_metrics"] = ["edge_concurrent_connection"]
-    ok, _, _, msg = DT.fits(flatten(payload), [0], 1)
+    ok, _, _, msg = twin.dist_fits(flatten(payload), [0], 1)
     assert not ok and "not sampled" in msg
 
 
@@ -197,7 +197,7 @@ def _results(values: np.ndarray, B: int) -> SweepResults:
 
 def test_group_dist_equals_numpy_on_the_values():
     rng = np.random.default_rng(7)
-    B = DT.gauge_bin(1 << 20) + 1
+    B = twin.gauge_bin(1 << 20) + 1
     for R in (1, 2, 7, 20, 101):
         small = rng.integers(0, 64, (R, 9))
         big = rng.integers(0, 1 << 20, (R, 9))
@@ -244,7 +244,7 @@ def test_shards_with_different_swept_ram_size_their_bins_differently():
     flat = flatten(load_scenario("c3_lb_two_servers.yml", 30))
     ram = [4096.0, 8192.0, 65536.0, 131072.0]
     col = ("server_ram_mb", flat.server_ids[0])
-    bins = [DT.fits(flat, [2], 2, request_capacity=16384, sweep=SweepSpec(flat, len(v), {col: v}))[2]
+    bins = [twin.dist_fits(flat, [2], 2, request_capacity=16384, sweep=SweepSpec(flat, len(v), {col: v}))[2]
             for v in (ram[:2], ram[2:], ram)]
     assert bins[0] < bins[1] == bins[2]
 
@@ -256,7 +256,7 @@ def test_concatenate_pads_shards_with_fewer_bins_and_checks_the_series():
     whole = _results(np.array([[1, 2], [70, 4], [5, 200]]), 120)
     np.testing.assert_array_equal(c.dist_hist, whole.dist_hist)
     d = c.group_dist("ready_queue_len", c.flat.server_ids[0], q=(0.5,))
-    np.testing.assert_array_equal(d["max"][0], gauge_bin_edges(120)[[DT.gauge_bin(70), DT.gauge_bin(200)]])
+    np.testing.assert_array_equal(d["max"][0], gauge_bin_edges(120)[[twin.gauge_bin(70), twin.gauge_bin(200)]])
     b.dist_series = [("ready_queue_len", b.flat.server_ids[-1] + "-other")]
     with pytest.raises(ValueError, match="different series"):
         SweepResults.concatenate([a, b])
@@ -278,7 +278,7 @@ def _gloo_part(rank: int) -> SweepResults:
     """Rank 0's shard sees values below 64 only (fewer bins), rank 1's up to 5 000 (more bins); both carry group sizes."""
     rng = np.random.default_rng(3 + rank)
     vals = rng.integers(0, 64 if rank == 0 else 5000, (7, 4))
-    r = _results(vals, DT.gauge_bin(int(vals.max())) + 1 + 3 * rank)
+    r = _results(vals, twin.gauge_bin(int(vals.max())) + 1 + 3 * rank)
     r.group_size = rng.integers(0, 1000, size=1).astype(np.int64)
     return r
 

@@ -5,9 +5,10 @@ the per-replica sampled sums; and no other output changes when bands are on."""
 
 from __future__ import annotations
 
-import band_twin as BT
+import band_ref
 import numpy as np
 import pytest
+import twin
 from helpers import SEED, load_scenario
 
 from asyncflow_b200 import Engine, EngineError, SweepRunner, SweepSpec, flatten
@@ -20,7 +21,7 @@ STOPS = K.FLAG_EVENT_OVERFLOW | K.FLAG_REQUEST_OVERFLOW | K.FLAG_NOWQ_OVERFLOW
 
 def traced_bands(eng: Engine, flat, n: int, groups: np.ndarray, n_groups: int):
     """Per-group sums of the device's own traced series (every replica traced, none stopped)."""
-    T, S = BT.ticks(flat), flat.n_series
+    T, S = twin.ticks(flat), flat.n_series
     cnt = np.zeros((n_groups, T), dtype=np.uint32)
     s = np.zeros((n_groups, S, T), dtype=np.uint64)
     sq = np.zeros((n_groups, S, T), dtype=np.uint64)
@@ -58,8 +59,8 @@ def test_device_bands_equal_traced_sums_and_the_twin(mode):
         assert (st["flags"] & STOPS == 0).all()
         got = eng.bands()
         assert_same(got, traced_bands(eng, flat, n, groups, G))
-    tw = BT.run_lane(flat, seed=SEED, n=n, sweep=spec, groups=groups, n_groups=G)
-    assert_same(got, BT.scan(flat, tw["band_rows"], G))
+    tw = twin.run_lane(flat, seed=SEED, n=n, sweep=spec, groups=groups, n_groups=G, sampled=True)
+    assert_same(got, band_ref.scan(flat, tw["band_rows"], G))
     assert (got[0] == n // G).all()
 
 
@@ -85,12 +86,13 @@ def test_two_pass_stitches_the_flagged_replicas():
     assert passes["lane_replicas"] > 0 and passes["warp_replicas"] > 0, passes
     assert (st["flags"] & STOPS == 0).all()
     assert_same(got, traced)
-    lane = BT.run_lane(flat, seed=SEED, n=n, groups=groups, n_groups=G, event_capacity=512, request_capacity=2048)
+    lane = twin.run_lane(flat, seed=SEED, n=n, groups=groups, n_groups=G, event_capacity=512, request_capacity=2048,
+                         sampled=True)
     flagged = np.flatnonzero(lane["stats"]["flags"] & STOPS)
     assert flagged.size == passes["warp_replicas"]
-    BT.run_warp(flat, seed=SEED, n=n, groups=groups, n_groups=G, event_capacity=ev_cap, request_capacity=rq_cap,
-                redo=flagged, band_from=lane["band_from"], into=lane)
-    assert_same(got, BT.scan(flat, lane["band_rows"], G))
+    twin.run_warp(flat, seed=SEED, n=n, groups=groups, n_groups=G, event_capacity=ev_cap, request_capacity=rq_cap,
+                redo=flagged, band_from=lane["band_from"], into=lane, sampled=True)
+    assert_same(got, band_ref.scan(flat, lane["band_rows"], G))
     assert (got[0] == n // G).all()
 
 
@@ -118,7 +120,7 @@ def test_bench_shape_band_totals_match_the_sampled_sums_and_change_nothing_else(
     for k in ("stats", "edge_sent", "edge_dropped", "samp_sum", "samp_max", "throughput"):
         assert getattr(r_on, k).tobytes() == getattr(r_off, k).tobytes(), k
     assert h_on.tobytes() == h_off.tobytes()
-    T = BT.ticks(on.flat)
+    T = twin.ticks(on.flat)
     assert r_on.band_count.shape == (G, T)
     assert not (r_on.stats["flags"] & K.FLAG_LB_EMPTY).any()
     assert (r_on.band_count == np.bincount(groups, minlength=G)[:, None]).all()

@@ -5,9 +5,10 @@ up across shards."""
 
 from __future__ import annotations
 
-import dist_twin as DT
+import band_ref
 import numpy as np
 import pytest
+import twin
 from helpers import ROOT, SEED, load_scenario
 
 from asyncflow_b200 import Engine, SweepRunner, flatten
@@ -79,8 +80,8 @@ def test_rows_are_the_histogram_of_the_traced_series(mode):
     np.testing.assert_array_equal(d, traced_hist(eng, n, series, groups, G, d.shape[3]))
     assert (d.sum(axis=3) == n // G).all()
     if mode == "two_pass":                          # the twin, both state machines
-        tw = DT.run_lane(flat, seed=SEED, n=n, series=series, groups=groups, n_groups=G)
-        np.testing.assert_array_equal(d, DT.scan(tw["dist_rows"], G, d.shape[2]))
+        tw = twin.run_lane(flat, seed=SEED, n=n, series=series, groups=groups, n_groups=G)
+        np.testing.assert_array_equal(d, band_ref.dist_scan(tw["dist_rows"], G, d.shape[2]))
 
 
 def test_a_stitched_launch_counts_each_replica_once():

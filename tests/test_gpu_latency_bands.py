@@ -6,9 +6,10 @@ pooled p95 agrees with numpy on the traced latencies."""
 
 from __future__ import annotations
 
-import latency_twin as LT
+import band_ref
 import numpy as np
 import pytest
+import twin
 from helpers import SEED, load_scenario
 
 from asyncflow_b200 import Engine, EngineError, SweepRunner, SweepSpec, flatten
@@ -20,14 +21,14 @@ STOPS = K.FLAG_EVENT_OVERFLOW | K.FLAG_REQUEST_OVERFLOW | K.FLAG_NOWQ_OVERFLOW |
 
 
 def traced_rows(eng: Engine, flat, n: int, groups: np.ndarray, n_groups: int, w: int) -> np.ndarray:
-    rows = LT.new_rows(flat, n_groups, w)
+    rows = twin.lat_rows(flat, n_groups, w)
     for i in range(n):
-        LT.bin_clocks(rows, int(groups[i]), eng.trace_clocks(i), w, int(flat.horizon_s))
+        band_ref.bin_clocks(rows, int(groups[i]), eng.trace_clocks(i), w, int(flat.horizon_s))
     return rows
 
 
 def assert_same(got, rows, n_groups):
-    want = LT.split(rows, n_groups)
+    want = twin.lat_split(rows, n_groups)
     for name, a, b in zip(("hist", "sum_hi", "sum_lo"), got, want):
         assert a.dtype == b.dtype and a.shape == b.shape and np.array_equal(a, b), name
 
@@ -51,7 +52,7 @@ def test_device_rows_equal_traced_clocks_and_the_twin(mode):
         assert (eng.stats()["flags"] & STOPS == 0).all()
         got = eng.latency_bands()
         assert_same(got, traced_rows(eng, flat, n, groups, G, w), G)
-    tw = LT.run_lane(flat, seed=SEED, n=n, sweep=spec, groups=groups, n_groups=G, window=w)
+    tw = twin.run_lane(flat, seed=SEED, n=n, sweep=spec, groups=groups, n_groups=G, window=w)
     assert_same(got, tw["lat_rows"], G)
 
 

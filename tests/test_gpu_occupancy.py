@@ -10,8 +10,8 @@ import subprocess
 import sys
 
 import numpy as np
-import occ_twin as OT
 import pytest
+import twin
 from helpers import ROOT, SEED, load_scenario
 
 from asyncflow_b200 import Engine, SweepRunner, flatten
@@ -59,7 +59,7 @@ def outputs(eng: Engine) -> dict:
 
 
 def twin_rows(flat, ids) -> np.ndarray:
-    return np.stack([OT.run_lane(flat, seed=SEED, n=1, replica_begin=int(i), f=F)["occ"][0] for i in ids])
+    return np.stack([twin.run_lane(flat, seed=SEED, n=1, replica_begin=int(i), f=F)["occ"][0] for i in ids])
 
 
 @pytest.mark.parametrize("mode", ["auto", "lane", "warp", "two_pass"])
@@ -69,7 +69,7 @@ def test_rows_equal_the_twin_on_a_multiwave_launch(mode):
     eng = launch(flat, n, mode=mode)
     occ, f = eng.occupancy()
     passes = eng.last_run_passes()
-    assert f == F and occ.shape == (n, OT.n_cols(flat))
+    assert f == F and occ.shape == (n, twin.occ_cols(flat))
     assert (eng.stats()["flags"] & STOPS == 0).all()
     if mode != "warp":
         assert passes["lane_pass"] == 1 and n > _sm_count() * passes["lane_warps_per_sm"] * 32, passes
@@ -87,7 +87,7 @@ def test_a_stitched_launch_gives_the_warp_pass_rows():
     assert passes["warp_replicas"] >= 1, passes
     assert two.occupancy()[0].tobytes() == warp.occupancy()[0].tobytes()
     ids = np.flatnonzero(np.arange(n) % 400 == 0)
-    rows = np.stack([OT.run_warp(flat, seed=SEED, n=1, replica_begin=int(i), f=F)["occ"][0] for i in ids])
+    rows = np.stack([twin.run_warp(flat, seed=SEED, n=1, replica_begin=int(i), f=F)["occ"][0] for i in ids])
     assert two.occupancy()[0][ids].tobytes() == rows.tobytes()
 
 

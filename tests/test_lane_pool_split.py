@@ -9,7 +9,6 @@ import ctypes as C
 import des_port
 import numpy as np
 import pytest
-import split_twin
 import twin
 from helpers import PARITY_CASES, SEED, assert_matches_oracle, load_scenario
 
@@ -34,7 +33,7 @@ def test_each_sweep_row_gets_the_split_of_its_own_load():
     payload = bench.workload(0, 6)
     flat = flatten(payload)
     spec = _c3_rtt_spec(flat, [0.001, 0.010, 0.025, 0.050])
-    pool, reported, rows = split_twin.row_splits(flat, spec, 604)
+    pool, reported, rows = twin.row_splits(flat, spec, 604)
     assert pool == 32
     needs = [r[0] for r in rows]
     assert needs == sorted(needs) and needs[0] <= 12 and needs[-1] >= 30, rows
@@ -61,10 +60,10 @@ def test_rows_with_very_different_splits_each_match_the_oracle():
     cores = np.array([1.0, 8.0, 1.0])
     spec = SweepSpec(flat, 3, {("users_mean",): users, ("server_cpu_cores", flat.server_ids[0]): cores})
     lane_bytes = 420
-    r = split_twin.run(flat, lane_bytes=lane_bytes, split="rows", seed=SEED, n=3, sweep=spec, trace=3, clock_cap=100000,
+    r = twin.run_lane(flat, lane_bytes=lane_bytes, split="rows", seed=SEED, n=3, sweep=spec, trace=3, clock_cap=100000,
                        request_capacity=200000)
     # the twin runs a warp of one lane: the same pool as 32 lanes of lane_bytes each
-    _, _, rows = split_twin.row_splits(flat, spec, lane_bytes)
+    _, _, rows = twin.row_splits(flat, spec, lane_bytes)
     st = r["stats"]
     for i in range(3):
         p = spec.payload_for(payload, i)
@@ -87,7 +86,7 @@ def test_random_per_replica_splits_match_the_oracle(name):
     shared memory), at budgets the CUDA engine runs: each replica equals the oracle."""
     payload = load_scenario(name, PARITY_CASES[name])
     flat = flatten(payload)
-    r = split_twin.run(flat, lane_bytes=520, split="random", split_seed=7, seed=SEED, replica_begin=5, n=3, trace=3,
+    r = twin.run_lane(flat, lane_bytes=520, split="random", split_seed=7, seed=SEED, replica_begin=5, n=3, trace=3,
                        clock_cap=300000, request_capacity=400000, event_capacity=8192)
     for i in range(3):
         o = des_port.simulate(payload, seed=SEED, replica=5 + i)

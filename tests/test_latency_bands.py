@@ -1,4 +1,4 @@
-"""CPU tier: per-window latency bands, through the CPU twin of both engines (tests/host_twin/af_latency_twin.cpp).
+"""CPU tier: per-window latency bands, through the CPU twin of both engines (tests/twin.py).
 
 The rows equal the oracle's clocks binned by finish window and latency bin, fixed-point sums included, in both state
 machines; a replica the thread-per-replica pass stops and the warp-per-replica pass re-runs from ``lat_from`` counts
@@ -12,11 +12,11 @@ from __future__ import annotations
 import math
 import socket
 
-import band_twin as BT
+import band_ref
 import des_port
-import latency_twin as LT
 import numpy as np
 import pytest
+import twin
 from helpers import PARITY_CASES, SEED, load_scenario
 
 from asyncflow_b200 import SweepResults, flatten
@@ -32,9 +32,9 @@ def oracle_clocks(payload, replica: int, seed: int = SEED) -> np.ndarray:
 
 
 def expected(flat, clocks: list[np.ndarray], groups, n_groups: int, w: int, upto=None) -> np.ndarray:
-    rows = LT.new_rows(flat, n_groups, w)
+    rows = twin.lat_rows(flat, n_groups, w)
     for i, (c, g) in enumerate(zip(clocks, groups)):
-        LT.bin_clocks(rows, int(g), c if upto is None else c[:int(upto[i])], w, int(flat.horizon_s))
+        band_ref.bin_clocks(rows, int(g), c if upto is None else c[:int(upto[i])], w, int(flat.horizon_s))
     return rows
 
 
@@ -53,8 +53,8 @@ def test_fixed_point_and_bins_match_the_python_definition():
     rng = np.random.default_rng(1)
     lats = np.concatenate([rng.exponential(0.05, 2000), [0.0, 2.0 ** -33, 3 * 2.0 ** -33, 1.0, 4096.5, 1e-9]])
     for lat in lats:
-        assert LT.lib().af_lat_twin_fixed32(float(lat)) == round(float(lat) * 4294967296.0)
-        assert LT.lib().af_lat_twin_hist_bin(float(lat)) == LT.hist_bin(float(lat))
+        assert twin.lib().af_twin_fixed32(float(lat)) == round(float(lat) * 4294967296.0)
+        assert twin.lib().af_twin_hist_bin(float(lat)) == band_ref.hist_bin(float(lat))
 
 
 @pytest.mark.parametrize("engine", ["lane", "warp"])
@@ -65,7 +65,7 @@ def test_latency_rows_equal_the_oracle_clocks_binned(name, engine):
     n, begin = 4, 2
     groups = np.array([1, 0, 1, 0], dtype=np.uint32)
     clocks = [oracle_clocks(payload, begin + i) for i in range(n)]
-    run = LT.run_lane if engine == "lane" else LT.run_warp
+    run = twin.run_lane if engine == "lane" else twin.run_warp
     for w in _widths(int(flat.horizon_s)):
         out = run(flat, seed=SEED, n=n, replica_begin=begin, groups=groups, n_groups=2, band_first=begin, window=w)
         assert (out["stats"]["flags"] & STOPS == 0).all()
@@ -89,16 +89,16 @@ def test_flagged_replicas_rerun_from_lat_from_give_the_first_hand_rows():
     n, seed = N_SMALL, SEED
     groups = (np.arange(n) % 3).astype(np.uint32)
     for w in (1, 7):
-        lane = LT.run_lane(flat, seed=seed, n=n, groups=groups, n_groups=3, window=w, sampled=True, **SMALL)
+        lane = twin.run_lane(flat, seed=seed, n=n, groups=groups, n_groups=3, window=w, sampled=True, **SMALL)
         st = lane["stats"]
         flagged = np.flatnonzero(st["flags"] & REDO)
         assert flagged.size >= 1
         assert ((lane["lat_from"][flagged] < st["completed"][flagged])).any(), "no completion after a flag"
-        out = LT.run_warp(flat, seed=seed, n=n, groups=groups, n_groups=3, window=w, sampled=True, redo=flagged, into=lane)
+        out = twin.run_warp(flat, seed=seed, n=n, groups=groups, n_groups=3, window=w, sampled=True, redo=flagged, into=lane)
         assert (out["stats"]["flags"] & STOPS == 0).all()
-        full = LT.run_warp(flat, seed=seed, n=n, groups=groups, n_groups=3, window=w, sampled=True)
+        full = twin.run_warp(flat, seed=seed, n=n, groups=groups, n_groups=3, window=w, sampled=True)
         assert_rows(out["lat_rows"], full["lat_rows"], 3)
-        assert np.array_equal(BT.scan(flat, out["band_rows"], 3)[1], BT.scan(flat, full["band_rows"], 3)[1])
+        assert np.array_equal(band_ref.scan(flat, out["band_rows"], 3)[1], band_ref.scan(flat, full["band_rows"], 3)[1])
         clocks = [oracle_clocks(payload, i, seed) for i in range(n)]
         assert_rows(out["lat_rows"], expected(flat, clocks, groups, 3, w), 3)
 
@@ -107,7 +107,7 @@ def test_a_stopped_replica_contributes_exactly_its_completions_before_the_stop()
     payload, flat = _overloaded()
     n, seed = N_SMALL, SEED
     groups = (np.arange(n) // 12).astype(np.uint32)
-    out = LT.run_lane(flat, seed=seed, n=n, groups=groups, n_groups=2, window=1, **SMALL)
+    out = twin.run_lane(flat, seed=seed, n=n, groups=groups, n_groups=2, window=1, **SMALL)
     st = out["stats"]
     stopped = (st["flags"] & STOPS) != 0
     assert stopped.any()
@@ -121,7 +121,7 @@ def test_a_stopped_replica_contributes_exactly_its_completions_before_the_stop()
 @pytest.mark.parametrize("engine", ["lane", "warp"])
 def test_latency_bands_change_no_other_output(engine):
     payload, flat = _overloaded()
-    run = LT.run_lane if engine == "lane" else LT.run_warp
+    run = twin.run_lane if engine == "lane" else twin.run_warp
     kw = dict(seed=SEED, n=5, replica_begin=1, groups=np.array([0, 1, 0, 1, 0], dtype=np.uint32), n_groups=2,
               band_first=1, trace=3, clock_cap=5000, event_capacity=24, request_capacity=12)
     if engine == "lane":
@@ -130,7 +130,7 @@ def test_latency_bands_change_no_other_output(engine):
     for sampled in (False, True):
         on = run(flat, window=3, sampled=sampled, **kw)
         assert (on["stats"]["flags"] & STOPS).any()
-        for k in BT.OUTPUTS:
+        for k in twin.OUTPUTS:
             assert on[k].tobytes() == off[k].tobytes(), k
         assert on["lat_rows"].any() and not off["lat_rows"].any()
         if sampled:       # and the per-tick bands are those of a run without latency bands
@@ -139,16 +139,16 @@ def test_latency_bands_change_no_other_output(engine):
 
 
 def test_window_and_row_size_checks():
-    ok, why = LT.fits(0, 60, 4, 1 << 40)
+    ok, why = twin.lat_fits(0, 60, 4, 1 << 40)
     assert not ok and "window of 0 s" in why
-    ok, why = LT.fits(-3, 60, 4, 1 << 40)
+    ok, why = twin.lat_fits(-3, 60, 4, 1 << 40)
     assert not ok and "window of -3 s" in why
-    assert LT.fits(1, 60, 1000, 80 << 30)[0]             # 1 001 x 60 x 4 098 x 8 B = 1.97 GB
-    ok, why = LT.fits(1, 60, 1000, 1 << 30)
+    assert twin.lat_fits(1, 60, 1000, 80 << 30)[0]             # 1 001 x 60 x 4 098 x 8 B = 1.97 GB
+    ok, why = twin.lat_fits(1, 60, 1000, 1 << 30)
     assert not ok and "1000 groups x 60 windows of 1 s need 1.97 GB of rows, more than the device's 1.07 GB" in why
-    ok, why = LT.fits(1, 86_400, 1_000_000, 80 << 30)
+    ok, why = twin.lat_fits(1, 86_400, 1_000_000, 80 << 30)
     assert not ok and "86400 windows" in why
-    assert LT.fits(7, 60, 3, 2 << 20)[0]                  # 4 x 9 windows x 4 098 x 8 B = 1.18 MB
+    assert twin.lat_fits(7, 60, 3, 2 << 20)[0]                  # 4 x 9 windows x 4 098 x 8 B = 1.18 MB
 
 
 def _old_global_percentile(histogram: np.ndarray, q: float) -> float:
@@ -252,10 +252,10 @@ def test_group_latency_statistics():
                      np.zeros((1, flat.n_series), np.uint32))
     lats = [rng.exponential(0.02, 500) + 0.001 for _ in range(4)]                 # group g, windows of 2 s over 5 s
     fins = [rng.uniform(0.0, 5.0, 500) for _ in range(4)]
-    rows = np.zeros((2, 3, LT.ROW), dtype=np.uint64)
+    rows = np.zeros((2, 3, twin.LAT_ROW), dtype=np.uint64)
     for g in range(2):
         for j in (2 * g, 2 * g + 1):
-            LT.bin_clocks(rows, g, np.stack([fins[j] - lats[j], fins[j]], axis=1), 2, 5)
+            band_ref.bin_clocks(rows, g, np.stack([fins[j] - lats[j], fins[j]], axis=1), 2, 5)
     r.lat_window_s, r.group_size = 2, np.array([2, 2])
     r.lat_hist, r.lat_sum_hi, r.lat_sum_lo = rows[:, :, :K.AF_HIST_BINS], rows[:, :, -2], rows[:, :, -1]
     out = r.group_latency()

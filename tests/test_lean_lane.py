@@ -5,24 +5,14 @@ rejects each feature the lean loop leaves out."""
 
 from __future__ import annotations
 
-import atexit
-import ctypes as C
-import shutil
-import subprocess
-import tempfile
-from pathlib import Path
-
 import numpy as np
 import pytest
+import twin
 from helpers import PARITY_CASES, SEED, load_scenario
+from twin import lean_qualifies as qualifies
 
 from asyncflow_b200 import SweepSpec, flatten
-from asyncflow_b200 import _capi as K
 
-_SRC = Path(__file__).resolve().parent / "host_twin" / "af_lean_twin.cpp"
-_lib = None
-OUTPUTS = ("stats", "sent", "dropped", "hist", "thr", "samp_sum", "samp_max", "trace_clocks", "trace_series",
-           "trace_counts")
 #: scenarios -> whether they qualify as written; the others run as one_endpoint() makes them
 SCENARIOS = {"c3_lb_two_servers.yml": True, "c1_my_service.yml": True, "chain_two_servers.yml": True,
              "tie_cpu_io.yml": False, "poisson_ties.yml": False, "overload_single.yml": False}
@@ -47,76 +37,10 @@ def scenario(name: str) -> dict:
     return payload if SCENARIOS[name] else one_endpoint(payload)
 
 
-def lib() -> C.CDLL:
-    global _lib
-    if _lib is None:
-        d = Path(tempfile.mkdtemp(prefix="af_lean_twin_"))
-        atexit.register(shutil.rmtree, d, True)
-        so = d / "libaf_lean_twin.so"
-        subprocess.run(["g++", "-O2", "-ffp-contract=off", "-std=c++17", "-fPIC", "-shared", "-x", "c++", "-o", str(so),
-                        str(_SRC)], check=True)
-        L = C.CDLL(str(so))
-        vp, u64, i32, u32 = C.c_void_p, C.c_uint64, C.c_int32, C.c_uint32
-        L.af_lean_twin_error.restype = C.c_char_p
-        L.af_lean_twin_trace_tick_capacity.argtypes = [C.POINTER(K.AfScenario)]
-        L.af_lean_twin_ticks.argtypes = [C.POINTER(K.AfScenario)]
-        L.af_lean_twin_ticks.restype = u32
-        L.af_lean_twin_qualifies.argtypes = [C.POINTER(K.AfScenario), i32]
-        L.af_lean_twin_run_lane.argtypes = [
-            C.POINTER(K.AfScenario), C.POINTER(K.AfSweep), C.POINTER(K.AfOptions), i32, i32, u64, u64, u64, u64,
-            i32, i32, i32, vp, u64, u64, u32, vp, vp, vp, vp] + [vp] * 10
-        _lib = L
-    return _lib
-
-
-def qualifies(flat, trace_replicas: int = 0) -> bool:
-    return bool(lib().af_lean_twin_qualifies(C.byref(flat.pod), trace_replicas))
-
-
-def run_lane(flat, *, lean: bool, n: int, sweep=None, split: int = 0, sampled: bool = False, window: int = 0,
-             lane_bytes: int = 604) -> dict:
-    """The thread-per-replica engine over replicas [0, n) in groups i % 3: ``split`` 0 = every replica on the
-    scenario's estimate, 1 = each sweep row on its own, 2 = a random split per replica."""
-    L = lib()
-    opt = K.AfOptions(2048, 16384, 0, 0, 1, 1, 0, 0)
-    ticks = int(L.af_lean_twin_ticks(C.byref(flat.pod)))
-    tick_cap = L.af_lean_twin_trace_tick_capacity(C.byref(flat.pod))
-    n_groups = 3
-    windows = -(-int(flat.horizon_s) // window) if window else 1
-    out = {
-        "stats": np.zeros(n, dtype=K.STATS_DTYPE),
-        "sent": np.zeros((n, flat.n_edges), dtype=np.uint32),
-        "dropped": np.zeros((n, flat.n_edges), dtype=np.uint32),
-        "hist": np.zeros((n, K.AF_HIST_BINS), dtype=np.uint32),
-        "thr": np.zeros((n, flat.horizon_s), dtype=np.uint32),
-        "samp_sum": np.zeros((n, flat.n_series), dtype=np.uint64),
-        "samp_max": np.zeros((n, flat.n_series), dtype=np.uint32),
-        "trace_clocks": np.zeros((1, 1, 2), dtype=np.float64),
-        "trace_series": np.zeros((1, flat.n_series, tick_cap), dtype=np.uint32),
-        "trace_counts": np.zeros((n, 2), dtype=np.uint32),
-        "band_rows": np.zeros((n_groups + 1, 1 + 2 * flat.n_series, ticks + 1), dtype=np.uint64),
-        "band_from": np.full(n, 0xFFFFFFFF, dtype=np.uint32),
-        "lat_rows": np.zeros((n_groups + 1, windows, K.AF_HIST_BINS + 2), dtype=np.uint64),
-        "lat_from": np.full(n, 0xFFFFFFFF, dtype=np.uint32),
-    }
-    groups = np.ascontiguousarray(np.arange(n) % n_groups, dtype=np.uint32)
-    sw_p, keep = None, None
-    if sweep is not None:
-        sw, keep = sweep.pod(0, None)
-        sw_p = C.byref(sw)
-    rc = L.af_lean_twin_run_lane(C.byref(flat.pod), sw_p, C.byref(opt), lane_bytes, split, 7, SEED, 0, n, int(lean),
-                                 int(sampled), int(window), groups.ctypes.data, 0, n, n_groups,
-                                 out["band_rows"].ctypes.data, out["band_from"].ctypes.data,
-                                 out["lat_rows"].ctypes.data, out["lat_from"].ctypes.data,
-                                 *[out[k].ctypes.data for k in OUTPUTS])
-    if rc != 0:
-        raise RuntimeError(L.af_lean_twin_error().decode())
-    del keep
-    return out
-
-
-def assert_lean_equals_full(flat, **kw) -> dict:
-    lean, full = run_lane(flat, lean=True, **kw), run_lane(flat, lean=False, **kw)
+def assert_lean_equals_full(flat, *, n: int, **kw) -> dict:
+    """The thread-per-replica engine over replicas [0, n) in groups i % 3, lean and full."""
+    kw.update(seed=SEED, n=n, groups=np.arange(n) % 3, n_groups=3, split_seed=7, lane_bytes=604)
+    lean, full = twin.run_lane(flat, lean=True, **kw), twin.run_lane(flat, lean=False, **kw)
     for k, v in full.items():
         assert v.tobytes() == lean[k].tobytes(), (k, kw)
     return lean
@@ -129,7 +53,7 @@ def test_lean_loop_equals_full_loop(name):
     flat = flatten(scenario(name))
     assert qualifies(flat)
     for sampled, lat in BANDS:
-        for split in (0, 2):
+        for split in ("scenario", "random"):
             out = assert_lean_equals_full(flat, n=6, split=split, sampled=sampled, window=2 if lat else 0)
             assert out["stats"]["completed"].sum() > 0
 
@@ -143,7 +67,7 @@ def test_lean_loop_equals_full_loop_on_bench_sweep_rows():
     ids = np.linspace(0, 99_999, 24).astype(np.int64)
     spec = SweepSpec(flat, ids.size, bench._c3_cols(flat, ids, 100_000))
     for sampled, lat in BANDS:
-        out = assert_lean_equals_full(flat, n=ids.size, sweep=spec, split=1, sampled=sampled, window=1 if lat else 0)
+        out = assert_lean_equals_full(flat, n=ids.size, sweep=spec, split="rows", sampled=sampled, window=1 if lat else 0)
         assert (out["stats"]["completed"] > 0).all()
 
 

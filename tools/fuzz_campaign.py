@@ -48,9 +48,8 @@ def one(seed: int):
         kw = dict(seed=SEED, replica_begin=seed, n=1, trace=1, clock_cap=200000, request_capacity=400000,
                   event_capacity=8192)
         layout = layout_for(seed)
-        if layout:          # tests/split_twin.py: the lane state machine with a split of its pool per replica
-            import split_twin
-            r = split_twin.run(flat, **kw, **layout)
+        if layout:          # the lane state machine with a split of its pool per replica
+            r = twin.run_lane(flat, **kw, **layout)
         else:
             r = twin.run(flat, engine=ENGINE, **kw)
         st = r["stats"][0]
@@ -76,10 +75,7 @@ def main() -> None:
     global ENGINE, BIG, LAYOUTS
     ENGINE, BIG, LAYOUTS = a.engine, a.big, a.layouts
     import twin
-    twin.build()
-    if LAYOUTS and ENGINE == "lane":
-        import split_twin
-        split_twin.lib()                # built once, before the workers fork
+    twin.lib()                          # built once, before the workers fork
     bad = []
     total = 0
     with mp.get_context("fork").Pool(a.jobs) as pool:

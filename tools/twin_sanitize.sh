@@ -7,14 +7,11 @@
 #   bash tools/twin_sanitize.sh [count]
 cd "$(dirname "$0")/.." || exit 1
 n=${1:-200}
-so=/tmp/libaf_host_twin_asan.so
+so=/tmp/libaf_twin_asan.so
 g++ -O1 -g -fsanitize=address,undefined -fno-omit-frame-pointer -ffp-contract=off -std=c++17 -fPIC -shared -x c++ \
-    -o $so tests/host_twin/af_host_twin.cpp || exit 1
-so2=/tmp/libaf_split_twin_asan.so
-g++ -O1 -g -fsanitize=address,undefined -fno-omit-frame-pointer -ffp-contract=off -std=c++17 -fPIC -shared -x c++ \
-    -o $so2 tests/host_twin/af_split_twin.cpp || exit 1
+    -o $so tests/host_twin/af_twin.cpp || exit 1
 export LD_PRELOAD=$(gcc -print-file-name=libasan.so):$(gcc -print-file-name=libubsan.so)
-export ASAN_OPTIONS=detect_leaks=0:halt_on_error=1 UBSAN_OPTIONS=print_stacktrace=1:halt_on_error=1 AF_TWIN_SO=$so AF_SPLIT_TWIN_SO=$so2
+export ASAN_OPTIONS=detect_leaks=0:halt_on_error=1 UBSAN_OPTIONS=print_stacktrace=1:halt_on_error=1 AF_TWIN_SO=$so
 python tools/fuzz_campaign.py --first 1500000 --count $n --jobs 1 --layouts &&
 python tools/fuzz_campaign.py --first 1510000 --count $((n / 10)) --jobs 1 --layouts --big &&
 python tools/fuzz_campaign.py --first 1520000 --count $((n / 2)) --jobs 1 --engine warp &&
