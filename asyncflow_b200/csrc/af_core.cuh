@@ -1284,7 +1284,7 @@ AF_IN void run_replica(State& W, uint64_t local_index, const BandArgs& band) {
         const double t = afr::u2d(m.tbits);
         const uint32_t payload = (uint32_t)m.key, ev_seq = (uint32_t)(m.key >> 32);
         W.busy = (W.busy & ~1u) | (m.more ? 1u : 0u);
-        {
+        if (!(W.flags & STOP_FLAGS)) {    // (arm_generator's timeout did not fit the pool: stop at the ticks taken so far)
             const double tick = W.tick_time;
             if (tick < t || (tick == t && W.tick_seq < ev_seq)) take_samples(W, t, ev_seq);
         }

@@ -1120,7 +1120,10 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
         if constexpr (kSampled) { if (AFL_UNLIKELY(dead)) band_stop(W, m); }     // before the frozen ticks to the horizon
         if constexpr (kLatency) { if (AFL_UNLIKELY(dead)) lat_stop(W, lat_g); }
         if constexpr (kDist) { if (AFL_UNLIKELY(dead)) dist_stop(W, m); }
-        if (run && !is_item) {
+        // A flag the generator phase raised in this iteration (its timeout did not fit the pool) stops the replica
+        // before its next tick: the ticks up to this event would miss the lost arrival, yet the stop (next iteration)
+        // would count them as exact, and af_run's second pass re-runs the replica only from there (band_from).
+        if (run && !is_item && (dead || !(W.flags & STOP_FLAGS))) {
             const double tick = W.tick_time;
             if (tick < t_ev || (tick == t_ev && W.tick_seq < ev_seq)) take_ticks<kLean>(W, m, t_ev, ev_seq);
         }

@@ -52,14 +52,17 @@ def light_heavy_rows(flat, n: int, seed: int) -> SweepSpec:
     return SweepSpec(flat, m, {("users_mean",): users, ("edge_mean", flat.edge_ids[1]): rtt})
 
 
-def device_run(eng: Engine, flat, n: int, *, sweep=None, trace: int = 0, clock_cap: int = 0, **opts) -> dict:
+def device_run(eng: Engine, flat, n: int, *, sweep=None, begin: int = BEGIN, rows: int | None = None, trace: int = 0,
+               clock_cap: int = 0, **opts) -> dict:
+    """Replicas [begin, begin + n); rows [begin, begin + rows) of ``sweep`` (default: one per replica) describe
+    replicas begin, ..."""
     eng.upload(flat)
     eng.configure(trace_replicas=trace, trace_clock_capacity=clock_cap, **opts)
     if sweep is not None:
-        eng.upload_sweep(sweep, BEGIN, row_first=BEGIN, row_count=n)
+        eng.upload_sweep(sweep, begin, row_first=begin, row_count=n if rows is None else rows)
     else:
         eng.upload_sweep(None)
-    eng.run(SEED, BEGIN, BEGIN + n)
+    eng.run(SEED, begin, begin + n)
     sent, dropped = eng.edge_counts()
     ssum, smax = eng.sampled()
     out = {"stats": eng.stats().copy(), "sent": sent, "dropped": dropped, "samp_sum": ssum, "samp_max": smax,
@@ -71,8 +74,9 @@ def device_run(eng: Engine, flat, n: int, *, sweep=None, trace: int = 0, clock_c
     return out
 
 
-def twin_run(flat, n: int, *, sweep=None, engine: str = "lane", **kw) -> dict:
-    return twin.run(flat, seed=SEED, replica_begin=BEGIN, n=n, sweep=sweep, sweep_first=BEGIN if sweep else 0,
+def twin_run(flat, n: int, *, sweep=None, begin: int = BEGIN, engine: str = "lane", **kw) -> dict:
+    """The twin over what :func:`device_run` runs: every row of ``sweep`` from ``begin`` on."""
+    return twin.run(flat, seed=SEED, replica_begin=begin, n=n, sweep=sweep, sweep_first=begin if sweep else 0,
                     engine=engine, **kw)
 
 
