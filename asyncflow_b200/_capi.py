@@ -11,7 +11,7 @@ from __future__ import annotations
 import ctypes as C
 from pathlib import Path
 
-AF_ABI_VERSION = 7
+AF_ABI_VERSION = 8
 AF_HIST_BINS = 4096
 AF_HIST_SUB_BITS = 7
 AF_HIST_MIN_EXP = -20
@@ -88,6 +88,10 @@ class AfSweep(C.Structure):
                 ("columns", C.POINTER(AfSweepColumn)), ("values", C.POINTER(C.c_double))]
 
 
+class AfTimeline(C.Structure):
+    _fields_ = [("n_rows", C.c_uint64), ("spikes", C.POINTER(AfSpikeMark)), ("outages", C.POINTER(AfOutageMark))]
+
+
 class AfOptions(C.Structure):
     _fields_ = [("event_capacity", C.c_int32), ("request_capacity", C.c_int32),
                 ("warps_per_block", C.c_int32), ("blocks_per_sm", C.c_int32),
@@ -143,6 +147,7 @@ EXPORTS = [
     "af_fetch_trace_series", "af_reduce_histograms", "af_engine_set_mode", "af_last_run_passes",
     "af_selftest_rng", "af_bands_upload", "af_fetch_bands", "af_bands_configure", "af_fetch_latency_bands",
     "af_dist_bands_configure", "af_fetch_dist_bands", "af_occupancy_configure", "af_fetch_occupancy",
+    "af_timeline_upload",
 ]
 
 _lib = None
@@ -170,6 +175,7 @@ def load() -> C.CDLL:
     lib.af_engine_configure.argtypes = [vp, C.POINTER(AfOptions)]
     lib.af_scenario_upload.argtypes = [vp, C.POINTER(AfScenario)]
     lib.af_sweep_upload.argtypes = [vp, C.POINTER(AfSweep), u64]
+    lib.af_timeline_upload.argtypes = [vp, C.POINTER(AfTimeline), u64]
     lib.af_run.argtypes = [vp, u64, u64, u64]
     lib.af_sync.argtypes = [vp]
     lib.af_last_run_ms.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(C.c_float)]

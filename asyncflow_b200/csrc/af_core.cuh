@@ -229,6 +229,13 @@ struct BandArgs {
     uint64_t* occ; double occ_scale;
 };
 
+// Per-replica timelines of a launch (af_sim_kernel's parameter; rows == 0: none): replica first + r, r < rows, copies its
+// marks from spikes + r * n_spike and outages + r * n_outage instead of Globals' tables (DESIGN.md §3.9).
+struct TimelineArgs {
+    const AfSpikeMark* spikes; const AfOutageMark* outages;
+    uint64_t first, rows;
+};
+
 constexpr int32_t NQ_CAP = 128;   // now-queue capacity (power of two)
 
 AF_IN int32_t align_up(int32_t x, int32_t a) { return (x + a - 1) / a * a; }
@@ -1086,7 +1093,8 @@ AF_IN void bind(State& W, unsigned char* ws, uint64_t warp_slot) {
     W.sp_rq_next = AF_G.spill_rq_next + warp_slot * rq_sp;
 }
 
-AF_FN void load_params(State& W) {
+// `spikes` / `outages`: the replica's mark tables (its timeline row, or the scenario's)
+AF_FN void load_params(State& W, const AfSpikeMark* spikes, const AfOutageMark* outages) {
     AF_SHARED(&W);
     const int lane = lane_id();
 #pragma unroll 1
@@ -1125,13 +1133,13 @@ AF_FN void load_params(State& W) {
     for (int32_t i = lane; i < AF_L.n_lb_edges; i += WARP) tbl_lb(W)[i] = (uint32_t)AF_G.lb_edges[i];
 #pragma unroll 1
     for (int32_t i = lane; i < AF_L.n_spike; i += WARP) {
-        const AfSpikeMark a = AF_G.spikes[i];
+        const AfSpikeMark a = spikes[i];
         SpikeS s; s.fire = a.fire_time; s.delta = a.delta; s.edge = (uint32_t)a.edge; s.pad = 0;
         tbl_spike(W)[i] = s;
     }
 #pragma unroll 1
     for (int32_t i = lane; i < AF_L.n_outage; i += WARP) {
-        const AfOutageMark a = AF_G.outages[i];
+        const AfOutageMark a = outages[i];
         OutageS o; o.fire = a.fire_time; o.lb_edge = a.lb_edge; o.down = a.down;
         tbl_outage(W)[i] = o;
     }
@@ -1205,7 +1213,7 @@ AF_FN void write_back(State& W) {
 // ---------------------------------------------------------------------------------
 // the replica
 // ---------------------------------------------------------------------------------
-AF_IN void run_replica(State& W, uint64_t local_index, const BandArgs& band) {
+AF_IN void run_replica(State& W, uint64_t local_index, const BandArgs& band, const TimelineArgs& tl) {
     W.local = local_index;
     W.replica = AF_G.replica_begin + local_index;
     W.now = 0.0; W.horizon = (double)AF_L.horizon_s; W.seq = 0;
@@ -1240,7 +1248,11 @@ AF_IN void run_replica(State& W, uint64_t local_index, const BandArgs& band) {
         }
     }
     w_sync();
-    load_params(W);
+    {
+        const uint64_t r = W.replica - tl.first;
+        const bool own = r < tl.rows;
+        load_params(W, own ? tl.spikes + r * (uint64_t)AF_L.n_spike : AF_G.spikes, own ? tl.outages + r * (uint64_t)AF_L.n_outage : AF_G.outages);
+    }
 
     // start order of the reference (simulation_runner.py:339-342, 301-336):
     // spike timeline, outage timeline, generator, ..., collector
@@ -1307,6 +1319,10 @@ AF_IN void run_replica(State& W, uint64_t local_index, const BandArgs& band) {
     if ((W.band != nullptr || W.dist != nullptr) && (W.flags & STOP_FLAGS)) band_stop(W);   // before the frozen ticks to the horizon
     take_samples(W, W.horizon, 0u);                   // ticks strictly before the horizon
     write_back(W);
+}
+AF_IN void run_replica(State& W, uint64_t local_index, const BandArgs& band) {
+    const TimelineArgs none = {};
+    run_replica(W, local_index, band, none);
 }
 AF_IN void run_replica(State& W, uint64_t local_index) {
     const BandArgs off = {};

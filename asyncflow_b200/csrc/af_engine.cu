@@ -62,7 +62,7 @@
 // ---------------------------------------------------------------------------------
 // kernels
 // ---------------------------------------------------------------------------------
-__global__ void AF_LAUNCH_BOUNDS af_sim_kernel(const afc::BandArgs band) {
+__global__ void AF_LAUNCH_BOUNDS af_sim_kernel(const afc::BandArgs band, const afc::TimelineArgs tl) {
     extern __shared__ __align__(16) unsigned char af_smem[];
     const int warp = (int)(threadIdx.x >> 5);
     const int lane = (int)(threadIdx.x & 31u);
@@ -80,7 +80,7 @@ __global__ void AF_LAUNCH_BOUNDS af_sim_kernel(const afc::BandArgs band) {
             r = afc::c_G.redo_list[r];
         } else if (r >= afc::c_G.n_replicas) break;
         else r = afc::c_G.order[r];
-        afc::run_replica(W, (uint64_t)r, band);
+        afc::run_replica(W, (uint64_t)r, band, tl);
         __syncwarp();
     }
 }
@@ -378,6 +378,10 @@ struct af_engine {
     std::vector<int32_t> h_row_need;               // aflh::row_events_estimates of the sweep's rows ...
     int32_t row_need_max = 0;                      // ... and the largest of them
     DevBuf d_sweep_cols, d_sweep_vals, d_row_need;
+    // per-replica timelines (af_timeline_upload): rows of replicas [tl_first, tl_first + tl_rows); the spike rows in both
+    // kernels' layouts (the warp kernel reads AfSpikeMark, the lane kernel afl::SpikeP), the outage rows in the one both read
+    uint64_t tl_rows = 0, tl_first = 0;
+    DevBuf d_tl_spikes, d_tl_l_spikes, d_tl_outages;
     // thread-per-replica pass: read-only tables (af_lane_host.h), global tiers, the list of flagged replicas
     int mode = AF_MODE_AUTO;
     aflh::Tables lt;
@@ -499,7 +503,7 @@ void af_engine_destroy(af_engine* e) {
                       &e->d_tclk, &e->d_tser, &e->d_tcnt, &e->d_counter, &e->d_htot,
                       &e->d_okey, &e->d_oidx, &e->d_order, &e->d_okey64, &e->d_sort_tmp,
                       &e->d_band_group, &e->d_band, &e->d_band_from, &e->d_lat, &e->d_lat_from,
-                      &e->d_dist_slot, &e->d_dist, &e->d_occ};
+                      &e->d_dist_slot, &e->d_dist, &e->d_occ, &e->d_tl_spikes, &e->d_tl_l_spikes, &e->d_tl_outages};
     for (DevBuf* b : bufs) b->release();
     cudaEventDestroy(e->ev_begin); cudaEventDestroy(e->ev_sim); cudaEventDestroy(e->ev_end);
     cudaStreamDestroy(e->stream);
@@ -544,6 +548,7 @@ int af_scenario_upload(af_engine* e, const AfScenario* s) {
     e->sc.outage_marks = e->h_outages.data();
     e->have_scenario = true;
     e->sweep_cols = 0; e->sweep_rows = 0; e->h_sweep_cols.clear();     // a sweep belongs to the scenario it was built for
+    e->tl_rows = 0;                                                     // ... and so do timeline rows
     e->ev_need = aflh::pending_events_estimate(e->sc, nullptr); e->row_need_max = 0;
     e->band_swept_ram = 0; e->band_swept_server = -1;
     e->ran = false;
@@ -619,6 +624,31 @@ int af_sweep_upload(af_engine* e, const AfSweep* sw, uint64_t first_replica) {
             "sweep row estimates H2D");
     AF_CUDA(e, cudaStreamSynchronize(e->stream), "sweep upload");
     e->sweep_cols = sw->n_columns; e->sweep_rows = sw->n_rows; e->sweep_first = first_replica;
+    return AF_OK;
+}
+
+int af_timeline_upload(af_engine* e, const AfTimeline* t, uint64_t first_replica) {
+    if (!e) return AF_ERR_INVALID;
+    if (!e->have_scenario) return e->fail(AF_ERR_STATE, "af_timeline_upload before af_scenario_upload");
+    if (!t || t->n_rows == 0) { e->tl_rows = 0; return AF_OK; }     // (a run in flight keeps the launch arguments it took)
+    AF_CUDA(e, cudaSetDevice(e->device), "cudaSetDevice");
+    AF_CUDA(e, cudaStreamSynchronize(e->stream), "sync before timeline upload");   // a run may still read the old rows
+    std::string why;
+    if (!afh::validate_timeline(e->sc, *t, why)) return e->fail(AF_ERR_INVALID, why);
+    const uint64_t ns = t->n_rows * (uint64_t)e->sc.n_spike_marks, no = t->n_rows * (uint64_t)e->sc.n_outage_marks;
+    std::vector<afl::SpikeP> lane_spikes;
+    aflh::timeline_spikes(e->sc, *t, lane_spikes);
+    AF_CUDA(e, e->d_tl_spikes.ensure(ns * sizeof(AfSpikeMark)), "timeline spike rows");
+    AF_CUDA(e, e->d_tl_l_spikes.ensure(ns * sizeof(afl::SpikeP)), "timeline spike rows");
+    AF_CUDA(e, e->d_tl_outages.ensure(no * sizeof(AfOutageMark)), "timeline outage rows");
+    if (ns) {
+        AF_CUDA(e, cudaMemcpyAsync(e->d_tl_spikes.p, t->spikes, ns * sizeof(AfSpikeMark), cudaMemcpyHostToDevice, e->stream), "timeline H2D");
+        AF_CUDA(e, cudaMemcpyAsync(e->d_tl_l_spikes.p, lane_spikes.data(), ns * sizeof(afl::SpikeP), cudaMemcpyHostToDevice, e->stream),
+                "timeline H2D");
+    }
+    if (no) AF_CUDA(e, cudaMemcpyAsync(e->d_tl_outages.p, t->outages, no * sizeof(AfOutageMark), cudaMemcpyHostToDevice, e->stream), "timeline H2D");
+    AF_CUDA(e, cudaStreamSynchronize(e->stream), "timeline upload");
+    e->tl_rows = t->n_rows; e->tl_first = first_replica;
     return AF_OK;
 }
 
@@ -768,6 +798,10 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
     AF_CUDA(e, cudaSetDevice(e->device), "cudaSetDevice");
     const uint64_t n = end - begin;
     int rc;
+    if (e->tl_rows) {
+        std::string why;
+        if (!afh::timeline_sweep_fits(e->h_sweep_cols.data(), e->sweep_cols, why)) return e->fail(AF_ERR_INVALID, why);
+    }
 
     // ---- pass structure ---------------------------------------------------------------------------------
     // AUTO: every replica runs on the thread-per-replica engine with tiers sized for nominal load; the ones
@@ -1005,6 +1039,11 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
     G.redo_count = redo ? (const uint32_t*)e->d_redo_count.p : nullptr;
     G.seed = seed; G.replica_begin = begin; G.n_replicas = n;
     if (occ) { band.occ = (uint64_t*)e->d_occ.p; band.occ_scale = ldexp(1.0, e->occ_opt.frac_bits); }
+    afc::TimelineArgs tl = {};
+    if (e->tl_rows) {
+        tl.spikes = (const AfSpikeMark*)e->d_tl_spikes.p; tl.outages = (const AfOutageMark*)e->d_tl_outages.p;
+        tl.first = e->tl_first; tl.rows = e->tl_rows;
+    }
     if (bands || lat || dist) { band.group = (const uint32_t*)e->d_band_group.p; band.first = e->band_first; band.n = e->h_band_group.size(); band.groups = e->band_groups; }
     if (dist) {
         band.from = (const uint32_t*)e->d_band_from.p;
@@ -1049,6 +1088,10 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
             C.lat_window = e->lat_window; C.lat_windows = (int32_t)lat_windows;
         }
         C.occ = band.occ;
+        if (e->tl_rows) {
+            C.tl_spikes = (const afl::SpikeP*)e->d_tl_l_spikes.p; C.tl_outages = (const afl::OutageP*)e->d_tl_outages.p;
+            C.tl_first = e->tl_first; C.tl_rows = e->tl_rows;
+        }
     }
 
     // ---- enqueue ---------------------------------------------------------------------------------------------------
@@ -1098,7 +1141,7 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
         AF_CUDA(e, cudaMemcpyToSymbolAsync(afc::c_L, &L, sizeof L, 0, cudaMemcpyHostToDevice, e->stream), "layout -> constant memory");
         e->G_host = G;   // keep the source alive until the async copy has been issued from pageable memory
         AF_CUDA(e, cudaMemcpyToSymbolAsync(afc::c_G, &e->G_host, sizeof G, 0, cudaMemcpyHostToDevice, e->stream), "globals -> constant memory");
-        af_sim_kernel<<<(unsigned)grid, wpb * 32, smem, e->stream>>>(band);
+        af_sim_kernel<<<(unsigned)grid, wpb * 32, smem, e->stream>>>(band, tl);
         AF_CUDA(e, cudaGetLastError(), "af_sim_kernel launch");
         e->launches += 1;
     }

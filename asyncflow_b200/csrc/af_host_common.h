@@ -81,6 +81,46 @@ inline bool validate(const AfScenario& s, std::string& err) {
     return true;
 }
 
+// The per-replica timeline rows of af_timeline_upload get the checks validate() applies to the scenario's tables, row by
+// row: spike edges in range, fire times non-decreasing, an outage's lb_edge -1 or one of the scenario's LB edges.
+inline bool validate_timeline(const AfScenario& s, const AfTimeline& t, std::string& err) {
+    char buf[256];
+#define AF_CHECK(cond, ...) do { if (!(cond)) { snprintf(buf, sizeof buf, __VA_ARGS__); err = buf; return false; } } while (0)
+    AF_CHECK((s.n_spike_marks == 0 || t.spikes) && (s.n_outage_marks == 0 || t.outages), "timeline: null mark rows");
+    for (uint64_t r = 0; r < t.n_rows; ++r) {
+        const AfSpikeMark* sp = t.spikes + r * (uint64_t)s.n_spike_marks;
+        for (int i = 0; i < s.n_spike_marks; ++i) {
+            AF_CHECK(sp[i].edge >= 0 && sp[i].edge < s.n_edges, "timeline row %llu: spike mark %d: edge %d out of range",
+                     (unsigned long long)r, i, sp[i].edge);
+            AF_CHECK(i == 0 || sp[i].fire_time >= sp[i - 1].fire_time, "timeline row %llu: spike marks unsorted at mark %d",
+                     (unsigned long long)r, i);
+        }
+        const AfOutageMark* om = t.outages + r * (uint64_t)s.n_outage_marks;
+        for (int i = 0; i < s.n_outage_marks; ++i) {
+            bool lb = om[i].lb_edge == -1;
+            for (int k = 0; k < s.n_lb_edges && !lb; ++k) lb = s.lb_edges[k] == om[i].lb_edge;
+            AF_CHECK(lb, "timeline row %llu: outage mark %d: lb_edge %d is neither -1 nor an edge of the load balancer",
+                     (unsigned long long)r, i, om[i].lb_edge);
+            AF_CHECK(i == 0 || om[i].fire_time >= om[i - 1].fire_time, "timeline row %llu: outage marks unsorted at mark %d",
+                     (unsigned long long)r, i);
+        }
+    }
+#undef AF_CHECK
+    return true;
+}
+
+// af_run's rule for a launch with timeline rows: no AF_FIELD_SPIKE_DELTA column (it indexes a mark in the scenario's
+// order, which a row may change; a row carries its own amplitudes).
+inline bool timeline_sweep_fits(const AfSweepColumn* cols, int32_t n_cols, std::string& err) {
+    for (int32_t c = 0; c < n_cols; ++c)
+        if (cols[c].field == AF_FIELD_SPIKE_DELTA) {
+            err = "af_run: sweep column " + std::to_string(c) + " sweeps a spike amplitude (AF_FIELD_SPIKE_DELTA) while timeline "
+                  "rows are uploaded; put the amplitudes in the rows' spike deltas";
+            return false;
+        }
+    return true;
+}
+
 inline int32_t trace_tick_capacity(const AfScenario& s) {
     double n = (double)s.horizon_s / s.sample_period;
     if (n > 50.0e6) n = 50.0e6;

@@ -192,6 +192,10 @@ struct Cfg {
     // write-back; occ_scale = 2^f (afr::occ_fixed)
     uint64_t* occ; double occ_scale;
     int32_t gi_occ, occ_cols;
+    // per-replica timelines (af_timeline_upload; DESIGN.md §3.9): replica tl_first + r, r < tl_rows, reads its marks at
+    // tl_spikes + r * n_spike and tl_outages + r * n_outage instead of spikes / outages (tl_rows = 0: none has a row)
+    const SpikeP* tl_spikes; const OutageP* tl_outages;
+    uint64_t tl_first, tl_rows;
 };
 
 
@@ -799,13 +803,23 @@ AFL_IN void ram_walk(St& W, const Mem& m, uint32_t sidx) {
     }
 }
 
-// ---- event injection (injection.py:167-226): all marks of this instant; returns true when the timeline re-arms
+// ---- event injection (injection.py:167-226): the replica's mark tables -- its timeline row, or the scenario's
+AFL_IN const SpikeP* spike_marks(const St& W) {
+    const uint64_t r = W.replica - AFL_C.tl_first;
+    return r < AFL_C.tl_rows ? AFL_C.tl_spikes + r * (uint64_t)AFL_C.n_spike : AFL_C.spikes;
+}
+AFL_IN const OutageP* outage_marks(const St& W) {
+    const uint64_t r = W.replica - AFL_C.tl_first;
+    return r < AFL_C.tl_rows ? AFL_C.tl_outages + r * (uint64_t)AFL_C.n_outage : AFL_C.outages;
+}
+// all marks of this instant; returns true when the timeline re-arms
 AFL_IN bool on_spike(St& W, const Mem& m, double& next_fire) {
+    const SpikeP* marks = spike_marks(W);
     int32_t cur = W.spike_cur;
-    const double t = ro(AFL_C.spikes + cur).fire;
+    const double t = ro(marks + cur).fire;
 #pragma unroll 1
     while (cur < AFL_C.n_spike) {
-        const SpikeP p = ro(AFL_C.spikes + cur);
+        const SpikeP p = ro(marks + cur);
         if (p.fire != t) break;
         double delta = p.delta;
         if (p.c_delta >= 0) { const double v = row_val(m, p.c_delta); delta = delta < 0.0 ? -v : v; }
@@ -813,17 +827,18 @@ AFL_IN bool on_spike(St& W, const Mem& m, double& next_fire) {
         ++cur;
     }
     W.spike_cur = cur;
-    if (cur < AFL_C.n_spike) { next_fire = ro(AFL_C.spikes + cur).fire; return true; }
+    if (cur < AFL_C.n_spike) { next_fire = ro(marks + cur).fire; return true; }
     return false;
 }
 AFL_IN bool on_outage(St& W, const Mem& m, double& next_fire) {
+    const OutageP* marks = outage_marks(W);
     int32_t cur = W.outage_cur;
-    const double t = ro(AFL_C.outages + cur).fire;
+    const double t = ro(marks + cur).fire;
     int32_t n = W.lb_n;
     const int32_t lb = AFL_C.o32_lb;
 #pragma unroll 1
     while (cur < AFL_C.n_outage) {
-        const OutageP p = ro(AFL_C.outages + cur);
+        const OutageP p = ro(marks + cur);
         if (p.fire != t) break;
         ++cur;
         if (p.lb_edge < 0) continue;
@@ -839,7 +854,7 @@ AFL_IN bool on_outage(St& W, const Mem& m, double& next_fire) {
     }
     W.lb_n = n;
     W.outage_cur = cur;
-    if (cur < AFL_C.n_outage) { next_fire = ro(AFL_C.outages + cur).fire; return true; }
+    if (cur < AFL_C.n_outage) { next_fire = ro(marks + cur).fire; return true; }
     return false;
 }
 
@@ -1031,13 +1046,13 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                 // start order of the reference (simulation_runner.py:339-342, 301-336):
                 // spike timeline, outage timeline, generator, ..., collector
                 if (!kLean && C.n_spike > 0) {
-                    double f = ro(C.spikes).fire;
+                    double f = ro(spike_marks(W)).fire;
                     bool arm = true;
                     if (f == 0.0) arm = on_spike(W, m, f);
                     if (arm && f < W.horizon) { if (f == W.now) W.busy |= 1u; heap_push(W, m, afr::d2u(f), ((uint64_t)(W.seq++) << 32) | mk_payload(K_SPIKE, 0, 0)); }
                 }
                 if (!kLean && C.n_outage > 0) {
-                    double f = ro(C.outages).fire;
+                    double f = ro(outage_marks(W)).fire;
                     bool arm = true;
                     if (f == 0.0) arm = on_outage(W, m, f);
                     if (arm && f < W.horizon) { if (f == W.now) W.busy |= 1u; heap_push(W, m, afr::d2u(f), ((uint64_t)(W.seq++) << 32) | mk_payload(K_OUTAGE, 0, 0)); }

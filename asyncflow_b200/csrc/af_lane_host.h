@@ -2,6 +2,7 @@
 // sweep's column map folded in, and the launch configuration (shared-memory layout of a warp, tier
 // sizes).  Shared by the CUDA engine (af_engine.cu) and the CPU-only debugging twin (tests/host_twin).
 #pragma once
+#include <stddef.h>
 #include <string>
 #include <vector>
 #include "af_lane.cuh"
@@ -80,6 +81,19 @@ inline bool build_tables(const AfScenario& s, const AfSweepColumn* cols, int32_t
     t.n_row = n_row;
     return true;
 }
+
+// Per-replica timeline rows (af_timeline_upload) in the lane kernel's layout: [n_rows][n_spike_marks] SpikeP with no
+// sweep slot (a row carries its own amplitudes).  The outage rows need no conversion: OutageP is AfOutageMark's layout.
+inline void timeline_spikes(const AfScenario& s, const AfTimeline& t, std::vector<afl::SpikeP>& out) {
+    const uint64_t n = t.n_rows * (uint64_t)s.n_spike_marks;
+    out.resize((size_t)n);
+    for (uint64_t i = 0; i < n; ++i) {
+        afl::SpikeP& p = out[(size_t)i];
+        p.fire = t.spikes[i].fire_time; p.delta = t.spikes[i].delta; p.edge = (uint32_t)t.spikes[i].edge; p.c_delta = -1; p.pad[0] = p.pad[1] = 0;
+    }
+}
+static_assert(sizeof(afl::OutageP) == sizeof(AfOutageMark) && offsetof(afl::OutageP, lb_edge) == offsetof(AfOutageMark, lb_edge)
+              && offsetof(afl::OutageP, down) == offsetof(AfOutageMark, down), "OutageP must be AfOutageMark's layout");
 
 // alias[c] = the first earlier column whose values equal column c's in every row, or -1
 inline std::vector<int32_t> column_aliases(const double* values, uint64_t n_rows, int32_t n_cols) {

@@ -81,13 +81,19 @@ class Engine:
 
     def upload_sweep(self, spec: SweepSpec | None, first_replica: int = 0, *, row_first: int = 0,
                      row_count: int | None = None) -> None:
-        """Rows ``[row_first, row_first+row_count)`` of ``spec`` describe replicas starting at ``first_replica``."""
+        """Rows ``[row_first, row_first+row_count)`` of ``spec`` describe replicas starting at ``first_replica``: its
+        columns (``af_sweep_upload``) and, when it sweeps event times, the same rows' timelines (``af_timeline_upload``;
+        otherwise the timeline rows are cleared).  ``None`` clears both."""
         if spec is None:
             self._check(self._lib.af_sweep_upload(self._h, None, 0), "af_sweep_upload")
+            self._check(self._lib.af_timeline_upload(self._h, None, 0), "af_timeline_upload")
             return
         sw, keep = spec.pod(row_first, row_count)
         self._check(self._lib.af_sweep_upload(self._h, C.byref(sw), int(first_replica)), "af_sweep_upload")
-        del keep
+        tl, keep_tl = spec.timeline_pod(row_first, row_count)
+        self._check(self._lib.af_timeline_upload(self._h, None if tl is None else C.byref(tl), int(first_replica)),
+                    "af_timeline_upload")
+        del keep, keep_tl
 
     # ------------------------------------------------------------------ run
     def run(self, seed: int, replica_begin: int, replica_end: int) -> None:

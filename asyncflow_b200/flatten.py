@@ -20,7 +20,8 @@ What the flattening resolves once, on the host, instead of per event:
 * the two injection timelines are sorted with the reference's key
   ``(t, mark == start, event_id, target_id)`` and their f64 FIRE times are
   accumulated exactly like ``dt = t - last_t; yield timeout(dt)`` does
-  (``runtime/events/injection.py:142-151,185-188``).
+  (``runtime/events/injection.py:142-151,185-188``) -- :func:`build_timelines`, which
+  also builds the per-row timelines of a sweep over event times.
 """
 
 from __future__ import annotations
@@ -54,12 +55,43 @@ def _as_dict(payload: Any) -> dict:
     raise TypeError(msg)
 
 
+#: numpy mirrors of AfSpikeMark / AfOutageMark: one row of mark tables per sweep row (af_timeline_upload)
+SPIKE_MARK_DTYPE = np.dtype([("fire_time", "<f8"), ("delta", "<f8"), ("edge", "<i4"), ("reserved", "<i4")])
+OUTAGE_MARK_DTYPE = np.dtype([("fire_time", "<f8"), ("lb_edge", "<i4"), ("down", "<i4")])
+assert SPIKE_MARK_DTYPE.itemsize == C.sizeof(K.AfSpikeMark) and OUTAGE_MARK_DTYPE.itemsize == C.sizeof(K.AfOutageMark)
+
+
 def _rv(d: dict) -> tuple[str, float, float]:
     dist = _s(d.get("distribution") or "poisson")
     var = d.get("variance")
     if var is None and dist in ("normal", "log_normal"):
         var = d["mean"]          # RVConfig.default_variance (schemas/common/random_variables.py)
     return dist, float(d["mean"]), 0.0 if var is None else float(var)
+
+
+@dataclass(frozen=True)
+class FlatEvent:
+    """One injected event, as :func:`build_timelines` needs it."""
+
+    event_id: str
+    target_id: str
+    spike: bool          # a network spike on an edge; else a server outage
+    target: int          # spike: the edge; outage: the load balancer's edge to the server, -1 when it covers none
+    server: int          # outage: the server; spike: -1
+    t_start: float
+    t_end: float
+    spike_s: float       # the spike's amplitude (0 for an outage)
+
+
+@dataclass
+class Timelines:
+    """Spike and outage mark tables of R rows (the layout of ``AfTimeline``), and which mark each entry is:
+    ``*_mark[r, j]`` = 2 k for the start of the k-th event of its kind (in payload order), 2 k + 1 for its end."""
+
+    spikes: np.ndarray          # [R, n_spike_marks] SPIKE_MARK_DTYPE
+    outages: np.ndarray         # [R, n_outage_marks] OUTAGE_MARK_DTYPE
+    spike_mark: np.ndarray      # [R, n_spike_marks] int64
+    outage_mark: np.ndarray     # [R, n_outage_marks] int64
 
 
 @dataclass
@@ -76,6 +108,8 @@ class FlatScenario:
     step_index: dict[tuple[str, int, int], int]        # (server, endpoint, original step idx) -> AfStep
     endpoint_index: dict[tuple[str, int], int]
     spike_mark_events: list[tuple[str, str]]           # (event_id, start|end) per AfSpikeMark
+    events: list[FlatEvent]                            # the spikes and outages, in payload order
+    lb_edges: list[int]
     horizon_s: int
     sample_period: float
     enabled_metrics: list[str]
@@ -94,18 +128,73 @@ class FlatScenario:
         return 3 * self.n_servers + self.n_edges
 
 
-def _timeline(marks: list[tuple[float, str, str, str]]) -> list[float]:
-    """Fire times of a sorted timeline: injection.py:178-188 in f64."""
-    now = 0.0
-    last_t = 0.0
-    out = []
-    for t, *_ in marks:
-        dt = t - last_t
-        if dt > 0.0:
-            now = now + dt
-        last_t = t
-        out.append(now)
-    return out
+def _sorted_fold(events: list[FlatEvent], t_start: np.ndarray, t_end: np.ndarray) -> tuple[np.ndarray, np.ndarray]:
+    """The marks of ``events`` (one kind) in every row, sorted with the reference's key ``(t, mark == start, event_id,
+    target_id)`` (a stable sort: equal keys keep payload order), and their FIRE times: injection.py:178-188 in f64,
+    ``dt = t - last_t; now += dt`` only when ``dt > 0``.  ``t_start`` / ``t_end``: [R, len(events)].
+    Returns (mark [R, 2k] as in :class:`Timelines`, fire [R, 2k])."""
+    R, k = t_start.shape[0], len(events)
+    t = np.empty((R, 2 * k))
+    t[:, 0::2], t[:, 1::2] = t_start, t_end
+    ids = [(e.event_id, e.target_id) for e in events]
+    rank = {key: i for i, key in enumerate(sorted(set(ids)))}
+    ev_rank = np.broadcast_to(np.repeat([rank[key] for key in ids], 2), t.shape)
+    is_start = np.broadcast_to(np.tile([True, False], k), t.shape)
+    mark = np.lexsort((ev_rank, is_start, t), axis=1) if k else np.zeros((R, 0), dtype=np.int64)
+    ts = np.take_along_axis(t, mark, axis=1)
+    fire = np.empty_like(ts)
+    now, last = np.zeros(R), np.zeros(R)
+    for j in range(2 * k):
+        dt = ts[:, j] - last
+        now = np.where(dt > 0.0, now + dt, now)
+        last = ts[:, j]
+        fire[:, j] = now
+    return mark.astype(np.int64), fire
+
+
+def build_timelines(events: list[FlatEvent], lb_edges: list[int], horizon: float, t_start: np.ndarray,
+                    t_end: np.ndarray, spike_s: np.ndarray, label=lambda r: "") -> Timelines:
+    """The spike and outage mark tables of R rows of event times (``t_start`` / ``t_end`` / ``spike_s``: [R, n_events],
+    columns in the order of ``events``): what ``flatten`` uploads for one row and ``SweepSpec`` for each of its rows.
+    Refuses (``ValueError``, prefixed by ``label(row)``) a row whose load balancer runs out of servers before the horizon."""
+    sp = [i for i, e in enumerate(events) if e.spike]
+    out = [i for i, e in enumerate(events) if not e.spike]
+    R = t_start.shape[0]
+    s_mark, s_fire = _sorted_fold([events[i] for i in sp], t_start[:, sp], t_end[:, sp])
+    spikes = np.zeros(s_mark.shape, dtype=SPIKE_MARK_DTYPE)
+    if sp:
+        ev = np.asarray(sp)[s_mark // 2]
+        amp = np.take_along_axis(spike_s, ev, axis=1)
+        spikes["fire_time"] = s_fire
+        spikes["delta"] = np.where(s_mark % 2 == 0, amp, -amp)
+        spikes["edge"] = np.asarray([e.target for e in events])[ev]
+    o_mark, o_fire = _sorted_fold([events[i] for i in out], t_start[:, out], t_end[:, out])
+    outages = np.zeros(o_mark.shape, dtype=OUTAGE_MARK_DTYPE)
+    if out:
+        ev = np.asarray(out)[o_mark // 2]
+        outages["fire_time"] = o_fire
+        outages["lb_edge"] = np.asarray([e.target for e in events])[ev]
+        outages["down"] = o_mark % 2 == 0
+    if lb_edges and out:                                # replay of the outage marks over the LB's edge set
+        pos = np.zeros(max(lb_edges) + 1, dtype=np.int64)      # LB edge -> its column of `up`
+        pos[lb_edges] = np.arange(len(lb_edges))
+        up = np.ones((R, len(lb_edges)), dtype=bool)
+        rows = np.arange(R)
+        for j in range(o_mark.shape[1]):
+            le, down = outages["lb_edge"][:, j], outages["down"][:, j] != 0
+            hit = le >= 0
+            up[rows[hit], pos[le[hit]]] = ~down[hit]
+            bad = np.flatnonzero(hit & ~up.any(axis=1) & (o_fire[:, j] < horizon))
+            if bad.size:
+                # The reference only rejects "all servers down" (schemas/payload.py:145-252); servers chained BEHIND a
+                # covered one keep that check quiet while the LB's own dict runs empty, and the first request that
+                # then reaches the LB dies in round_robin (routing/lb_algorithms.py:22-36).  Say so up front.
+                r = int(bad[0])
+                e = events[out[int(o_mark[r, j]) // 2]]
+                msg = (f"{label(r)}event injection: at t={o_fire[r, j]:g}s every server behind the load balancer is down "
+                       f"(mark {e.event_id!r} on {e.target_id!r}); the reference's load balancer raises on an empty edge set")
+                raise ValueError(msg)
+    return Timelines(spikes, outages, s_mark, o_mark)
 
 
 def flatten(payload: Any) -> FlatScenario:
@@ -208,42 +297,27 @@ def flatten(payload: Any) -> FlatScenario:
         lb_algo = K.LB_ROUND_ROBIN if algo == "round_robin" else K.LB_LEAST_CONNECTIONS
 
     # ---- event injection (runtime/events/injection.py:112-164) ---------------
-    e_tl: list[tuple[float, str, str, str]] = []
-    s_tl: list[tuple[float, str, str, str]] = []
-    spike_of: dict[tuple[str, str], float] = {}
-    for ev in events:
-        st, en = ev["start"], ev["end"]
-        a = (float(st["t_start"]), ev["event_id"], ev["target_id"], "start")
-        b = (float(en["t_end"]), ev["event_id"], ev["target_id"], "end")
-        if ev["target_id"] in eidx:
-            spike_of[(ev["event_id"], ev["target_id"])] = float(st["spike_s"])
-            e_tl += [a, b]
-        elif ev["target_id"] in sidx:
-            s_tl += [a, b]
-    key = lambda m: (m[0], m[3] == "start", m[1], m[2])  # noqa: E731
-    e_tl.sort(key=key)
-    s_tl.sort(key=key)
     edge_by_server: dict[str, int] = {}
     for i in lb_edges:                                  # injection.py:158-164
         edge_by_server[edges[i]["target"]] = i
-    c_spikes = (K.AfSpikeMark * max(1, len(e_tl)))()
-    for i, (m, fire) in enumerate(zip(e_tl, _timeline(e_tl))):
-        amp = spike_of[(m[1], m[2])]
-        c_spikes[i] = K.AfSpikeMark(fire, amp if m[3] == "start" else -amp, eidx[m[2]], 0)
-    c_out = (K.AfOutageMark * max(1, len(s_tl)))()
-    pool = set(lb_edges)                                # replay of the outage marks over the LB's edge set
-    for i, (m, fire) in enumerate(zip(s_tl, _timeline(s_tl))):
-        le = edge_by_server.get(m[2], -1)
-        c_out[i] = K.AfOutageMark(fire, le, 1 if m[3] == "start" else 0)
-        if le >= 0:
-            pool.discard(le) if m[3] == "start" else pool.add(le)
-            if lb_edges and not pool and fire < horizon:
-                # The reference only rejects "all servers down" (schemas/payload.py:145-252); servers chained BEHIND a
-                # covered one keep that check quiet while the LB's own dict runs empty, and the first request that
-                # then reaches the LB dies in round_robin (routing/lb_algorithms.py:22-36).  Say so up front.
-                msg = (f"event injection: at t={fire:g}s every server behind the load balancer is down "
-                       f"(mark {m[1]!r} on {m[2]!r}); the reference's load balancer raises on an empty edge set")
-                raise ValueError(msg)
+    flat_events: list[FlatEvent] = []
+    for ev in events:
+        st, en = ev["start"], ev["end"]
+        tgt = ev["target_id"]
+        if tgt in eidx:
+            flat_events.append(FlatEvent(ev["event_id"], tgt, True, eidx[tgt], -1, float(st["t_start"]),
+                                         float(en["t_end"]), float(st["spike_s"])))
+        elif tgt in sidx:
+            flat_events.append(FlatEvent(ev["event_id"], tgt, False, edge_by_server.get(tgt, -1), sidx[tgt],
+                                         float(st["t_start"]), float(en["t_end"]), 0.0))
+    tl = build_timelines(flat_events, lb_edges, horizon, np.array([[e.t_start for e in flat_events]]),
+                         np.array([[e.t_end for e in flat_events]]), np.array([[e.spike_s for e in flat_events]]))
+    c_spikes = (K.AfSpikeMark * max(1, tl.spikes.shape[1]))()
+    C.memmove(c_spikes, tl.spikes.tobytes(), tl.spikes.nbytes)
+    c_out = (K.AfOutageMark * max(1, tl.outages.shape[1]))()
+    C.memmove(c_out, tl.outages.tobytes(), tl.outages.nbytes)
+    spike_events = [e for e in flat_events if e.spike]
+    spike_mark_events = [(spike_events[m // 2].event_id, "start" if m % 2 == 0 else "end") for m in tl.spike_mark[0]]
 
     pod = K.AfScenario()
     pod.users_dist = K.DIST[udist]
@@ -258,7 +332,7 @@ def flatten(payload: Any) -> FlatScenario:
     pod.n_endpoints, pod.n_steps = len(eps), len(steps)
     pod.n_lb_edges, pod.lb_algo = len(lb_edges), lb_algo
     pod.gen_edge, pod.client_edge = out_edge_of(gen_id), out_edge_of(client_id)
-    pod.n_spike_marks, pod.n_outage_marks = len(e_tl), len(s_tl)
+    pod.n_spike_marks, pod.n_outage_marks = tl.spikes.shape[1], tl.outages.shape[1]
     pod.edges = C.cast(c_edges, C.POINTER(K.AfEdge))
     pod.servers = C.cast(c_servers, C.POINTER(K.AfServer))
     pod.endpoints = C.cast(c_eps, C.POINTER(K.AfEndpoint))
@@ -271,7 +345,8 @@ def flatten(payload: Any) -> FlatScenario:
         pod=pod, edge_ids=edge_ids, server_ids=server_ids, client_id=client_id,
         generator_id=gen_id, lb_id=lb_id, endpoint_names=ep_names, step_index=step_index,
         endpoint_index=endpoint_index,
-        spike_mark_events=[(m[1], m[3]) for m in e_tl], horizon_s=horizon, sample_period=period,
+        spike_mark_events=spike_mark_events, events=flat_events, lb_edges=lb_edges, horizon_s=horizon,
+        sample_period=period,
         enabled_metrics=enabled,
         _keep=[c_edges, c_servers, c_eps, c_steps, c_lb, c_spikes, c_out],
     )
@@ -313,18 +388,35 @@ class SweepSpec:
     (requests per second per user), ``("edge_mean"|"edge_sigma"|"edge_dropout", edge_id)``,
     ``("server_cpu_cores"|"server_ram_mb", server_id)``,
     ``("step_duration", server_id, endpoint_idx, step_idx)``,
-    ``("endpoint_ram", server_id, endpoint_idx)``, ``("spike_delta", event_id)``.
+    ``("endpoint_ram", server_id, endpoint_idx)``, ``("spike_delta", event_id)``,
+    ``("event_start"|"event_end", event_id)`` (the ``t_start`` / ``t_end`` of a spike or an outage).
+
+    A spec that sweeps an event time gives every row its own spike and outage timelines (:attr:`timelines`, uploaded
+    with the sweep): the marks sorted and their fire times folded as ``flatten`` does for the scenario, a row's
+    ``spike_delta`` folded into its marks' amplitudes.  Each row must pass the reference's payload rules --
+    ``0 <= t_start < t_end <= horizon``, no two outages of one server overlapping, not every server down at once --
+    and keep a server behind the load balancer up until the horizon; a row that does not is refused with a
+    ``ValueError`` naming the row, the event and the rule.
     """
 
     def __init__(self, flat: FlatScenario, n_replicas: int, columns: dict[tuple, Any]) -> None:
         self.n_replicas = int(n_replicas)
         self.selectors: list[tuple[tuple, np.ndarray]] = []
+        self.timelines: Timelines | None = None
         cols: list[tuple[int, int]] = []
         vals: list[np.ndarray] = []
-        for sel, v in columns.items():
-            sel = tuple(sel) if not isinstance(sel, str) else (sel,)
+        keys = [tuple(sel) if not isinstance(sel, str) else (sel,) for sel in columns]
+        times = any(k[0] in ("event_start", "event_end") for k in keys)
+        event_of = {e.event_id: i for i, e in enumerate(flat.events)}
+        for sel, v in zip(keys, columns.values()):
             name = sel[0]
             arr = np.ascontiguousarray(np.broadcast_to(np.asarray(v, dtype=np.float64), (self.n_replicas,)))
+            if name in ("event_start", "event_end") or (times and name == "spike_delta"):
+                if sel[1] not in event_of or (name == "spike_delta" and not flat.events[event_of[sel[1]]].spike):
+                    msg = f"no {'spike ' if name == 'spike_delta' else ''}event {sel[1]!r}"
+                    raise KeyError(msg)
+                self.selectors.append((sel, arr))       # carried by the rows' timelines, not by a column
+                continue
             if name in ("users_mean", "users_sigma", "rate_per_user"):
                 targets = [0]
             elif name.startswith("edge_"):
@@ -352,6 +444,70 @@ class SweepSpec:
                        else np.zeros((self.n_replicas, 0)))
         self._cols = (K.AfSweepColumn * max(1, len(cols)))(*[K.AfSweepColumn(f, i) for f, i in cols])
         self.columns = cols
+        if times:
+            self.timelines = self._timelines(flat)
+
+    def _timelines(self, flat: FlatScenario) -> Timelines:
+        """Every row's event times and amplitudes, checked against the payload rules, then its mark tables."""
+        ev = flat.events
+        R, E = self.n_replicas, len(ev)
+        field = {"event_start": "t_start", "event_end": "t_end", "spike_delta": "spike_s"}
+        cols = {f: np.tile(np.array([getattr(e, f) for e in ev], dtype=np.float64), (R, 1)) for f in field.values()}
+        index = {e.event_id: i for i, e in enumerate(ev)}
+        for sel, arr in self.selectors:
+            if sel[0] in field:
+                cols[field[sel[0]]][:, index[sel[1]]] = arr
+        ts, te, amp = cols["t_start"], cols["t_end"], cols["spike_s"]
+        H = float(flat.horizon_s)
+
+        def refuse(bad: np.ndarray, e: int, rule: str) -> None:
+            r = int(np.flatnonzero(bad)[0])
+            msg = (f"sweep row {r}: event {ev[e].event_id!r} (t_start={float(ts[r, e])!r}, t_end={float(te[r, e])!r}"
+                   f"{f', spike_s={float(amp[r, e])!r}' if ev[e].spike else ''}): {rule}")
+            raise ValueError(msg)
+
+        for e in range(E):                      # schemas/events/injection.py:88, schemas/payload.py:64-104
+            ok = (ts[:, e] >= 0.0) & (ts[:, e] < te[:, e]) & (te[:, e] <= H)
+            if not ok.all():
+                refuse(~ok, e, f"an event needs 0 <= t_start < t_end <= the horizon ({H:g} s)")
+            if ev[e].spike and not (np.isfinite(amp[:, e]) & (amp[:, e] >= 0.0)).all():
+                refuse(~(np.isfinite(amp[:, e]) & (amp[:, e] >= 0.0)), e, "a spike's spike_s is finite and >= 0")
+        by_server: dict[int, list[int]] = {}
+        for e, x in enumerate(ev):
+            if not x.spike:
+                by_server.setdefault(x.server, []).append(e)
+        for evs in by_server.values():           # payload.py:203-252 (back to back is fine: END sorts before START)
+            for i, a in enumerate(evs):
+                for b in evs[i + 1:]:
+                    both = (ts[:, a] < te[:, b]) & (ts[:, b] < te[:, a])
+                    if both.any():
+                        refuse(both, b, f"overlaps the outage {ev[a].event_id!r} of the same server")
+        if len(by_server) == flat.n_servers:     # payload.py:145-200: at some outage's start every server is down
+            for e0 in (e for evs in by_server.values() for e in evs):
+                t = ts[:, e0]
+                down = np.ones(R, dtype=bool)
+                for evs in by_server.values():
+                    down &= np.any([(ts[:, e] <= t) & (t < te[:, e]) for e in evs], axis=0)
+                if down.any():
+                    refuse(down, e0, "every server is down once it starts; keep at least one up")
+        return build_timelines(ev, flat.lb_edges, H, ts, te, amp, label=lambda r: f"sweep row {r}: ")
+
+    def timeline_pod(self, first: int = 0, count: int | None = None) -> tuple[K.AfTimeline | None, Any]:
+        """AfTimeline over rows ``[first, first+count)`` (``None`` when the spec sweeps no event time); keep the returned
+        arrays alive."""
+        if self.timelines is None:
+            return None, None
+        count = self.n_replicas - first if count is None else count
+        sp = np.ascontiguousarray(self.timelines.spikes[first:first + count])
+        ou = np.ascontiguousarray(self.timelines.outages[first:first + count])
+        tl = K.AfTimeline(count, sp.ctypes.data_as(C.POINTER(K.AfSpikeMark)), ou.ctypes.data_as(C.POINTER(K.AfOutageMark)))
+        return tl, (sp, ou)
+
+    @property
+    def timeline_row_bytes(self) -> int:
+        """Bytes of one row's timelines (0 without)."""
+        tl = self.timelines
+        return 0 if tl is None else tl.spikes.shape[1] * tl.spikes.itemsize + tl.outages.shape[1] * tl.outages.itemsize
 
     def estimated_cost(self, flat: FlatScenario) -> np.ndarray:
         """Expected arrivals per row (users x rate x horizon): the load proxy ``balanced_order`` sorts by."""
@@ -416,6 +572,13 @@ class SweepSpec:
                 for ev in p.get("events") or []:
                     if ev["event_id"] == sel[1]:
                         ev["start"]["spike_s"] = v
+            elif name in ("event_start", "event_end"):
+                for ev in p.get("events") or []:
+                    if ev["event_id"] == sel[1]:
+                        if name == "event_start":
+                            ev["start"]["t_start"] = v
+                        else:
+                            ev["end"]["t_end"] = v
         return p
 
     def pin(self) -> None:

@@ -38,7 +38,7 @@
 extern "C" {
 #endif
 
-#define AF_ABI_VERSION 7
+#define AF_ABI_VERSION 8
 
 typedef enum AfStatus {
     AF_OK = 0,
@@ -217,6 +217,23 @@ int af_engine_set_mode(af_engine* e, int mode);
 int af_scenario_upload(af_engine* e, const AfScenario* host_pod);
 /* rows cover replicas [first_replica, first_replica + sweep->n_rows); pass NULL to clear */
 int af_sweep_upload(af_engine* e, const AfSweep* sweep, uint64_t first_replica);
+
+/* Per-replica event timelines: row r replaces the scenario's spike and outage mark tables for replica
+ * first_replica + r; replicas outside [first_replica, first_replica + n_rows) keep the scenario's, as with sweep rows.
+ * A row holds the scenario's number of marks of each kind (n_spike_marks, n_outage_marks), under the contract of
+ * AfScenario's tables: sorted by the reference's key, fire times already folded, spike deltas signed.  Only the order,
+ * times, amplitudes and targets may differ from row to row (an outage moved across another one reorders the marks).
+ * af_timeline_upload refuses (AF_ERR_INVALID, naming the row) a spike mark whose edge is out of range, fire times that
+ * decrease within a row, and an outage mark whose lb_edge is neither -1 nor one of the scenario's lb_edges.  NULL (or
+ * n_rows = 0) clears the rows; af_scenario_upload clears them too.  af_run refuses (AF_ERR_INVALID) a launch with
+ * timeline rows and an AF_FIELD_SPIKE_DELTA sweep column: that column indexes a mark in the scenario's order, which a
+ * row may change, so a row carries its amplitudes in its own deltas. */
+typedef struct AfTimeline {
+    uint64_t n_rows;
+    const AfSpikeMark* spikes;   /* [n_rows][n_spike_marks]                                            */
+    const AfOutageMark* outages; /* [n_rows][n_outage_marks]                                           */
+} AfTimeline;
+int af_timeline_upload(af_engine* e, const AfTimeline* timeline, uint64_t first_replica);
 
 /* Simulate replicas [replica_begin, replica_end) start to horizon.  Asynchronous
  * on the engine's stream; af_sync / any af_fetch_* waits for it.                 */
