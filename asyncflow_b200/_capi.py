@@ -11,7 +11,7 @@ from __future__ import annotations
 import ctypes as C
 from pathlib import Path
 
-AF_ABI_VERSION = 8
+AF_ABI_VERSION = 9
 AF_HIST_BINS = 4096
 AF_HIST_SUB_BITS = 7
 AF_HIST_MIN_EXP = -20
@@ -147,7 +147,7 @@ EXPORTS = [
     "af_fetch_trace_series", "af_reduce_histograms", "af_engine_set_mode", "af_last_run_passes",
     "af_selftest_rng", "af_bands_upload", "af_fetch_bands", "af_bands_configure", "af_fetch_latency_bands",
     "af_dist_bands_configure", "af_fetch_dist_bands", "af_occupancy_configure", "af_fetch_occupancy",
-    "af_timeline_upload",
+    "af_timeline_upload", "af_streams_upload",
 ]
 
 _lib = None
@@ -176,6 +176,7 @@ def load() -> C.CDLL:
     lib.af_scenario_upload.argtypes = [vp, C.POINTER(AfScenario)]
     lib.af_sweep_upload.argtypes = [vp, C.POINTER(AfSweep), u64]
     lib.af_timeline_upload.argtypes = [vp, C.POINTER(AfTimeline), u64]
+    lib.af_streams_upload.argtypes = [vp, vp, u64, u64]
     lib.af_run.argtypes = [vp, u64, u64, u64]
     lib.af_sync.argtypes = [vp]
     lib.af_last_run_ms.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(C.c_float)]

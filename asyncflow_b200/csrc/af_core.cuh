@@ -148,7 +148,7 @@ struct State {
     // behind this struct: see tbl_*() below -- 32-bit shared addresses, no pointer loads)
     double* sp_ev_time; uint64_t* sp_ev_key; ReqRec* sp_rq_rec; uint32_t* sp_rq_next;
     // identity
-    uint64_t replica, local;
+    uint64_t replica, local;                // replica: the stream its draws are keyed by; local: its output slot
     // clock + pending-event pool
     double now, horizon;
     uint32_t seq;
@@ -233,6 +233,13 @@ struct BandArgs {
 // marks from spikes + r * n_spike and outages + r * n_outage instead of Globals' tables (DESIGN.md §3.9).
 struct TimelineArgs {
     const AfSpikeMark* spikes; const AfOutageMark* outages;
+    uint64_t first, rows;
+};
+
+// Random streams of a launch (af_sim_kernel's parameter; rows == 0: none): replica first + i, i < rows, draws as
+// stream_of[i], every other replica as its own id (DESIGN.md §3.10).
+struct StreamArgs {
+    const uint64_t* stream_of;
     uint64_t first, rows;
 };
 
@@ -1151,7 +1158,7 @@ AF_FN void load_params(State& W, const AfSpikeMark* spikes, const AfOutageMark* 
     w_sync();
     W.users_mean = AF_L.users_mean; W.users_sigma = AF_L.users_sigma; W.rate_per_user = AF_L.rate_per_user;
     // sweep overrides of this replica (uniform: every lane applies every column)
-    const uint64_t replica = W.replica;
+    const uint64_t replica = AF_G.replica_begin + W.local;     // (W.replica is its stream)
     if (AF_L.n_sweep_cols > 0 && replica >= AF_G.sweep_first && replica - AF_G.sweep_first < AF_G.sweep_rows) {
         const double* row = AF_G.sweep_vals + (replica - AF_G.sweep_first) * (uint64_t)AF_L.n_sweep_cols;
 #pragma unroll 1
@@ -1213,9 +1220,11 @@ AF_FN void write_back(State& W) {
 // ---------------------------------------------------------------------------------
 // the replica
 // ---------------------------------------------------------------------------------
-AF_IN void run_replica(State& W, uint64_t local_index, const BandArgs& band, const TimelineArgs& tl) {
+AF_IN void run_replica(State& W, uint64_t local_index, const BandArgs& band, const TimelineArgs& tl, const StreamArgs& rs) {
     W.local = local_index;
-    W.replica = AF_G.replica_begin + local_index;
+    const uint64_t id = AF_G.replica_begin + local_index;     // the replica's rows; its draws come from its stream
+    const uint64_t si = id - rs.first;
+    W.replica = si < rs.rows ? rs.stream_of[si] : id;
     W.now = 0.0; W.horizon = (double)AF_L.horizon_s; W.seq = 0;
     W.ev_hw = 0; W.ev_live = 0; W.ev_last_free = -1; W.ev_hole = -1; W.peak_ev = 0;
     W.nq_head = 0; W.nq_tail = 0; W.busy = 0;
@@ -1236,7 +1245,7 @@ AF_IN void run_replica(State& W, uint64_t local_index, const BandArgs& band, con
         for (int32_t c = lane_id(); c < cols; c += WARP) W.occ[c] = 0;
     }
     if (band.stride || band.lat_window || band.dist_rows) {
-        const uint64_t i = W.replica - band.first;
+        const uint64_t i = id - band.first;
         const uint32_t g = i < band.n ? band.group[i] : band.groups;
         if (band.stride || band.dist_rows)                           // a re-run continues where the lane pass stopped
             W.band_from = AF_G.redo_list ? band.from[local_index] : 0u;
@@ -1249,7 +1258,7 @@ AF_IN void run_replica(State& W, uint64_t local_index, const BandArgs& band, con
     }
     w_sync();
     {
-        const uint64_t r = W.replica - tl.first;
+        const uint64_t r = id - tl.first;
         const bool own = r < tl.rows;
         load_params(W, own ? tl.spikes + r * (uint64_t)AF_L.n_spike : AF_G.spikes, own ? tl.outages + r * (uint64_t)AF_L.n_outage : AF_G.outages);
     }
@@ -1319,6 +1328,10 @@ AF_IN void run_replica(State& W, uint64_t local_index, const BandArgs& band, con
     if ((W.band != nullptr || W.dist != nullptr) && (W.flags & STOP_FLAGS)) band_stop(W);   // before the frozen ticks to the horizon
     take_samples(W, W.horizon, 0u);                   // ticks strictly before the horizon
     write_back(W);
+}
+AF_IN void run_replica(State& W, uint64_t local_index, const BandArgs& band, const TimelineArgs& tl) {
+    const StreamArgs none = {};
+    run_replica(W, local_index, band, tl, none);
 }
 AF_IN void run_replica(State& W, uint64_t local_index, const BandArgs& band) {
     const TimelineArgs none = {};

@@ -62,7 +62,7 @@
 // ---------------------------------------------------------------------------------
 // kernels
 // ---------------------------------------------------------------------------------
-__global__ void AF_LAUNCH_BOUNDS af_sim_kernel(const afc::BandArgs band, const afc::TimelineArgs tl) {
+__global__ void AF_LAUNCH_BOUNDS af_sim_kernel(const afc::BandArgs band, const afc::TimelineArgs tl, const afc::StreamArgs rs) {
     extern __shared__ __align__(16) unsigned char af_smem[];
     const int warp = (int)(threadIdx.x >> 5);
     const int lane = (int)(threadIdx.x & 31u);
@@ -80,7 +80,7 @@ __global__ void AF_LAUNCH_BOUNDS af_sim_kernel(const afc::BandArgs band, const a
             r = afc::c_G.redo_list[r];
         } else if (r >= afc::c_G.n_replicas) break;
         else r = afc::c_G.order[r];
-        afc::run_replica(W, (uint64_t)r, band, tl);
+        afc::run_replica(W, (uint64_t)r, band, tl, rs);
         __syncwarp();
     }
 }
@@ -166,12 +166,13 @@ __global__ void af_flagged_kernel(const AfReplicaStats* __restrict__ stats, uint
 // A lane runs replicas back to back, and the launch ends when its last lane does.  Pulled in id order, the heaviest
 // replicas of a sweep tend to come last and the launch ends on a few busy lanes; the simulation kernels therefore pull
 // local indices through an order: heaviest first by each replica's predicted work (DESIGN.md §3.3).  Which lane runs a
-// replica, and when, changes no result: its random numbers are keyed by its replica id, its outputs by its local index.
+// replica, and when, changes no result: its random numbers are keyed by its stream, its outputs by its local index.
 struct OrderArgs {
     const AfSweepColumn* cols; const double* vals; int32_t n_cols; uint64_t sweep_first, sweep_rows;
     const int32_t* row_need; int32_t need;     // per-row pending-events estimates (nullptr: `need` for every replica)
     uint64_t seed, begin, n;
     int32_t users_dist; double users_mean, users_sigma, rate_per_user, span;   // span: the first window, at most the horizon
+    const uint64_t* stream_of; uint64_t stream_first, stream_rows;             // af_streams_upload's table (rows 0: none)
 };
 
 // the replica's pending-events estimate: its row's, else the scenario's
@@ -190,7 +191,8 @@ __global__ void af_order_key_kernel(const OrderArgs a, uint32_t* __restrict__ ke
     double um = a.users_mean, us = a.users_sigma, rate = a.rate_per_user;
     if (r < a.sweep_rows)
         for (int32_t c = 0; c < a.n_cols; ++c) afl::gen_field(a.cols[c].field, a.vals[r * (uint64_t)a.n_cols + (uint64_t)c], um, us, rate);
-    const double users = afr::gen_users(a.seed, replica, 0u, a.users_dist, um, us).value;
+    const uint64_t si = replica - a.stream_first;                    // the draw the replica makes: from its stream
+    const double users = afr::gen_users(a.seed, si < a.stream_rows ? a.stream_of[si] : replica, 0u, a.users_dist, um, us).value;
     const double cost = users * rate * a.span * (AF_ORDER_EVENT_COST + (double)order_need(a, i));
     key[i] = cost > 0.0 ? __float_as_uint((float)cost) : 0u;
     idx[i] = (uint32_t)i;
@@ -382,6 +384,9 @@ struct af_engine {
     // kernels' layouts (the warp kernel reads AfSpikeMark, the lane kernel afl::SpikeP), the outage rows in the one both read
     uint64_t tl_rows = 0, tl_first = 0;
     DevBuf d_tl_spikes, d_tl_l_spikes, d_tl_outages;
+    // random streams (af_streams_upload): replica stream_first + i, i < stream_rows, draws as d_streams[i]
+    uint64_t stream_rows = 0, stream_first = 0;
+    DevBuf d_streams;
     // thread-per-replica pass: read-only tables (af_lane_host.h), global tiers, the list of flagged replicas
     int mode = AF_MODE_AUTO;
     aflh::Tables lt;
@@ -503,7 +508,7 @@ void af_engine_destroy(af_engine* e) {
                       &e->d_tclk, &e->d_tser, &e->d_tcnt, &e->d_counter, &e->d_htot,
                       &e->d_okey, &e->d_oidx, &e->d_order, &e->d_okey64, &e->d_sort_tmp,
                       &e->d_band_group, &e->d_band, &e->d_band_from, &e->d_lat, &e->d_lat_from,
-                      &e->d_dist_slot, &e->d_dist, &e->d_occ, &e->d_tl_spikes, &e->d_tl_l_spikes, &e->d_tl_outages};
+                      &e->d_dist_slot, &e->d_dist, &e->d_occ, &e->d_tl_spikes, &e->d_tl_l_spikes, &e->d_tl_outages, &e->d_streams};
     for (DevBuf* b : bufs) b->release();
     cudaEventDestroy(e->ev_begin); cudaEventDestroy(e->ev_sim); cudaEventDestroy(e->ev_end);
     cudaStreamDestroy(e->stream);
@@ -649,6 +654,18 @@ int af_timeline_upload(af_engine* e, const AfTimeline* t, uint64_t first_replica
     if (no) AF_CUDA(e, cudaMemcpyAsync(e->d_tl_outages.p, t->outages, no * sizeof(AfOutageMark), cudaMemcpyHostToDevice, e->stream), "timeline H2D");
     AF_CUDA(e, cudaStreamSynchronize(e->stream), "timeline upload");
     e->tl_rows = t->n_rows; e->tl_first = first_replica;
+    return AF_OK;
+}
+
+int af_streams_upload(af_engine* e, const uint64_t* stream_of, uint64_t n, uint64_t first_replica) {
+    if (!e) return AF_ERR_INVALID;
+    if (!stream_of || n == 0) { e->stream_rows = 0; return AF_OK; }   // (a run in flight keeps the launch arguments it took)
+    AF_CUDA(e, cudaSetDevice(e->device), "cudaSetDevice");
+    AF_CUDA(e, cudaStreamSynchronize(e->stream), "sync before stream upload");     // a run may still read the old table
+    AF_CUDA(e, e->d_streams.ensure(n * sizeof(uint64_t)), "stream table");
+    AF_CUDA(e, cudaMemcpyAsync(e->d_streams.p, stream_of, n * sizeof(uint64_t), cudaMemcpyHostToDevice, e->stream), "stream table H2D");
+    AF_CUDA(e, cudaStreamSynchronize(e->stream), "stream upload");
+    e->stream_rows = n; e->stream_first = first_replica;
     return AF_OK;
 }
 
@@ -1018,6 +1035,7 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
     oa.users_dist = e->sc.users_dist; oa.users_mean = e->sc.users_mean; oa.users_sigma = e->sc.users_sigma;
     oa.rate_per_user = e->sc.rate_per_user;
     oa.span = (double)(e->sc.window_s < e->sc.horizon_s ? e->sc.window_s : e->sc.horizon_s);   // only the first window is predicted
+    if (e->stream_rows) { oa.stream_of = (const uint64_t*)e->d_streams.p; oa.stream_first = e->stream_first; oa.stream_rows = e->stream_rows; }
 
     afc::Globals G;
     memset(&G, 0, sizeof G);
@@ -1044,6 +1062,8 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
         tl.spikes = (const AfSpikeMark*)e->d_tl_spikes.p; tl.outages = (const AfOutageMark*)e->d_tl_outages.p;
         tl.first = e->tl_first; tl.rows = e->tl_rows;
     }
+    afc::StreamArgs rs = {};
+    if (e->stream_rows) { rs.stream_of = (const uint64_t*)e->d_streams.p; rs.first = e->stream_first; rs.rows = e->stream_rows; }
     if (bands || lat || dist) { band.group = (const uint32_t*)e->d_band_group.p; band.first = e->band_first; band.n = e->h_band_group.size(); band.groups = e->band_groups; }
     if (dist) {
         band.from = (const uint32_t*)e->d_band_from.p;
@@ -1092,6 +1112,7 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
             C.tl_spikes = (const afl::SpikeP*)e->d_tl_l_spikes.p; C.tl_outages = (const afl::OutageP*)e->d_tl_outages.p;
             C.tl_first = e->tl_first; C.tl_rows = e->tl_rows;
         }
+        C.stream_of = rs.stream_of; C.stream_first = rs.first; C.stream_rows = rs.rows;
     }
 
     // ---- enqueue ---------------------------------------------------------------------------------------------------
@@ -1141,7 +1162,7 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
         AF_CUDA(e, cudaMemcpyToSymbolAsync(afc::c_L, &L, sizeof L, 0, cudaMemcpyHostToDevice, e->stream), "layout -> constant memory");
         e->G_host = G;   // keep the source alive until the async copy has been issued from pageable memory
         AF_CUDA(e, cudaMemcpyToSymbolAsync(afc::c_G, &e->G_host, sizeof G, 0, cudaMemcpyHostToDevice, e->stream), "globals -> constant memory");
-        af_sim_kernel<<<(unsigned)grid, wpb * 32, smem, e->stream>>>(band, tl);
+        af_sim_kernel<<<(unsigned)grid, wpb * 32, smem, e->stream>>>(band, tl, rs);
         AF_CUDA(e, cudaGetLastError(), "af_sim_kernel launch");
         e->launches += 1;
     }

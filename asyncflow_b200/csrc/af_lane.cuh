@@ -196,6 +196,11 @@ struct Cfg {
     // tl_spikes + r * n_spike and tl_outages + r * n_outage instead of spikes / outages (tl_rows = 0: none has a row)
     const SpikeP* tl_spikes; const OutageP* tl_outages;
     uint64_t tl_first, tl_rows;
+    // random streams (af_streams_upload; DESIGN.md §3.10): replica stream_first + i, i < stream_rows, draws as
+    // stream_of[i], every other replica as its own id.  W.replica holds the stream; the rows a replica reads (sweep,
+    // pool estimate, band group, timeline) are addressed by its id, replica_begin + W.local.
+    const uint64_t* stream_of;
+    uint64_t stream_first, stream_rows;
 };
 
 
@@ -292,7 +297,7 @@ AFL_IN void st_t64(const Mem& m, int32_t os, int32_t gi, int32_t idx, int32_t sp
 
 // the replica's scalar state: registers (nothing here is indexed dynamically)
 struct St {
-    uint64_t replica, local;
+    uint64_t replica, local;                    // replica: the stream its draws are keyed by; local: its output slot
     double now, horizon;
     uint32_t seq; int32_t ev_n; uint32_t peak_ev;
     uint64_t arr_t; uint32_t arr_seq, arr_on;   // the generator's pending timeout: always exactly one, kept out of the heap
@@ -679,7 +684,7 @@ AFL_IN void take_ticks(St& W, const Mem& m, double t, uint32_t ev_seq) {
 //      frozen ticks to the horizon add nothing.  Every tick before n_ticks was taken before the event in which the
 //      flag was raised: those are exact, and the warp-per-replica pass re-runs the replica from that tick (band_from).
 AFL_IN void band_start(St& W) {
-    const uint64_t i = W.replica - AFL_C.band_first;
+    const uint64_t i = AFL_C.replica_begin + W.local - AFL_C.band_first;
     const uint32_t g = i < AFL_C.band_n ? AFL_C.band_group[i] : (uint32_t)AFL_C.band_groups;
     W.band = AFL_C.band_rows + (uint64_t)g * AFL_C.band_group_words;
     red_add64(W.band, 1u);
@@ -708,7 +713,7 @@ AFL_IN void band_stop(const St& W, const Mem& m) {
 //      kernels without latency bands keep the exact code they had before.
 constexpr uint32_t LAT_OFF = ~0u;
 AFL_IN uint32_t lat_group(const St& W) {
-    const uint64_t i = W.replica - AFL_C.band_first;
+    const uint64_t i = AFL_C.replica_begin + W.local - AFL_C.band_first;
     return i < AFL_C.band_n ? AFL_C.band_group[i] : (uint32_t)AFL_C.band_groups;
 }
 AFL_IN void lat_add(const St& W, uint32_t& lat_g, uint32_t done, double lat) {
@@ -805,11 +810,11 @@ AFL_IN void ram_walk(St& W, const Mem& m, uint32_t sidx) {
 
 // ---- event injection (injection.py:167-226): the replica's mark tables -- its timeline row, or the scenario's
 AFL_IN const SpikeP* spike_marks(const St& W) {
-    const uint64_t r = W.replica - AFL_C.tl_first;
+    const uint64_t r = AFL_C.replica_begin + W.local - AFL_C.tl_first;
     return r < AFL_C.tl_rows ? AFL_C.tl_spikes + r * (uint64_t)AFL_C.n_spike : AFL_C.spikes;
 }
 AFL_IN const OutageP* outage_marks(const St& W) {
-    const uint64_t r = W.replica - AFL_C.tl_first;
+    const uint64_t r = AFL_C.replica_begin + W.local - AFL_C.tl_first;
     return r < AFL_C.tl_rows ? AFL_C.tl_outages + r * (uint64_t)AFL_C.n_outage : AFL_C.outages;
 }
 // all marks of this instant; returns true when the timeline re-arms
@@ -899,7 +904,7 @@ template <bool kLean>
 AFL_IN void start_replica(St& W, const Mem& m, uint64_t local_index) {
     const Cfg& C = AFL_C;
     W.local = local_index;
-    W.replica = C.replica_begin + local_index;
+    W.replica = C.replica_begin + local_index;       // its id until the end: the rows below are the id's
     W.now = 0.0; W.horizon = (double)C.horizon_s; W.seq = 0;
     W.ev_n = 0; W.peak_ev = 0; W.arr_t = 0; W.arr_seq = 0; W.arr_on = 0;
     W.nq_head = 0; W.nq_tail = 0; W.busy = 0;
@@ -961,6 +966,8 @@ AFL_IN void start_replica(St& W, const Mem& m, uint64_t local_index) {
         if (C.collect_hist) for (int32_t b = 0; b < AF_HIST_BINS; ++b) C.hist[W.local * AF_HIST_BINS + (uint32_t)b] = 0;
         if (C.collect_thr) for (int32_t b = 0; b < C.horizon_s; ++b) C.thr[W.local * (uint64_t)C.horizon_s + (uint32_t)b] = 0;
     }
+    const uint64_t si = W.replica - C.stream_first;   // from here on W.replica is the stream the replica draws from
+    if (si < C.stream_rows) W.replica = C.stream_of[si];
 }
 
 template <bool kLean>

@@ -95,6 +95,16 @@ class Engine:
                     "af_timeline_upload")
         del keep, keep_tl
 
+    def upload_streams(self, streams, first_replica: int = 0) -> None:
+        """Replica ``first_replica + i`` draws its random numbers as stream ``streams[i]`` (u64) from the next run on;
+        every other replica as its own id.  ``None`` clears the table (``af_streams_upload``)."""
+        if streams is None:
+            self._check(self._lib.af_streams_upload(self._h, None, 0, 0), "af_streams_upload")
+            return
+        s = np.ascontiguousarray(streams, dtype=np.uint64)
+        self._check(self._lib.af_streams_upload(self._h, s.ctypes.data if s.size else None, s.size, int(first_replica)),
+                    "af_streams_upload")
+
     # ------------------------------------------------------------------ run
     def run(self, seed: int, replica_begin: int, replica_end: int) -> None:
         self._check(self._lib.af_run(self._h, int(seed), int(replica_begin), int(replica_end)), "af_run")

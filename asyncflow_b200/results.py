@@ -298,6 +298,7 @@ class SweepResults:
         self.histograms = histograms
         self.replica_begin = replica_begin
         self.rows: np.ndarray | None = None      # sweep row of each result row (set by SweepRunner)
+        self.streams: np.ndarray | None = None   # random stream of each result row (SweepRunner.stream_ids; set by collect)
         self.traced: list[ReplicaResults] = []    # full clocks + sampled series of the first `trace_replicas` replica ids
         self.exact: np.ndarray | None = None      # rows whose p50/p95/p99 are exact (SweepRunner.exact_percentiles)
         # per-tick bands (SweepRunner(bands=...)): per group g, series j, tick k: replicas that contribute the tick,
@@ -368,18 +369,28 @@ class SweepResults:
         t = np.maximum(self.stats["n_ticks"], 1).astype(np.float64)[:, None]
         return self.samp_sum.astype(np.float64) / t
 
-    def confidence_interval(self, what: str = "mean", select: np.ndarray | None = None,
-                            level: float = 0.95) -> tuple[float, float, float]:
-        """Monte-Carlo estimate over replicas of a per-replica statistic (``"mean"``, ``"p50"``,
-        ``"p95"``, ``"p99"``, ``"completed"``, ``"generated"``): ``(estimate, lo, hi)`` with a normal
-        ``level`` interval on the mean across the selected replicas (reference ROADMAP.md:23-27)."""
-        if what == "mean":
-            x = self.mean_latency
-        elif what in ("p50", "p95", "p99", "completed", "generated", "lat_min", "lat_max"):
-            x = self.stats[what].astype(np.float64)
-        else:
+    def _statistic(self, what: Any) -> np.ndarray:
+        """A per-replica statistic as f64: ``"mean"`` (latency), ``"p50"``, ``"p95"``, ``"p99"``, ``"completed"``,
+        ``"generated"``, ``"lat_min"``, ``"lat_max"``, or any array of one float per result row (e.g. ``time_in(...)``)."""
+        if isinstance(what, str):
+            if what == "mean":
+                return self.mean_latency
+            if what in ("p50", "p95", "p99", "completed", "generated", "lat_min", "lat_max"):
+                return self.stats[what].astype(np.float64)
             msg = f"unknown statistic {what!r}"
             raise KeyError(msg)
+        x = np.asarray(what, dtype=np.float64)
+        if x.shape != (len(self),):
+            msg = f"a statistic has one value per result row ({len(self)}), got shape {x.shape}"
+            raise ValueError(msg)
+        return x
+
+    def confidence_interval(self, what: Any = "mean", select: np.ndarray | None = None,
+                            level: float = 0.95) -> tuple[float, float, float]:
+        """Monte-Carlo estimate over replicas of a per-replica statistic (a name or an array, see :meth:`_statistic`):
+        ``(estimate, lo, hi)`` with a normal ``level`` interval on the mean across the selected replicas (reference
+        ROADMAP.md:23-27)."""
+        x = self._statistic(what)
         if select is not None:
             x = x[select]
         x = x[np.isfinite(x)]
@@ -392,6 +403,46 @@ class SweepResults:
         z = NormalDist().inv_cdf(0.5 + level / 2.0)
         half = z * float(x.std(ddof=1)) / float(np.sqrt(x.size))
         return m, m - half, m + half
+
+    def paired(self, what: Any, a, b, level: float = 0.95) -> dict[str, Any]:
+        """Paired comparison of two alternatives: the mean of ``x[a] - x[b]`` over the pairs ``(a[k], b[k])`` of result
+        rows, ``x`` a statistic as :meth:`confidence_interval` takes it.  Rows that share a random stream
+        (``SweepRunner(streams=)``) see the same traffic, so their difference cancels most of the noise both share
+        (common random numbers).  Pairs
+        with a non-finite side are dropped.  Returns ``estimate``, ``lo``, ``hi`` (the normal ``level`` interval of the
+        mean difference), ``half_width``, ``n`` (pairs kept), ``corr`` (correlation of the two sides), and
+        ``unpaired`` = ``(estimate, lo, hi)`` with ``unpaired_half_width``: the interval of the same difference had the
+        two sides been independent (``sqrt(var_a / n + var_b / n)``), so the gain of the pairing is visible."""
+        x = self._statistic(what)
+        a = np.atleast_1d(np.asarray(a, dtype=np.int64))
+        b = np.atleast_1d(np.asarray(b, dtype=np.int64))
+        if a.shape != b.shape or a.ndim != 1:
+            msg = f"paired: a and b are row-index arrays of one length, got shapes {a.shape} and {b.shape}"
+            raise ValueError(msg)
+        xa, xb = x[a], x[b]
+        keep = np.isfinite(xa) & np.isfinite(xb)
+        xa, xb = xa[keep], xb[keep]
+        n = int(xa.size)
+        nan = float("nan")
+        out: dict[str, Any] = {"estimate": nan, "lo": nan, "hi": nan, "half_width": nan, "n": n, "corr": nan,
+                               "unpaired": (nan, nan, nan), "unpaired_half_width": nan}
+        if n == 0:
+            return out
+        d = xa - xb
+        m = float(d.mean())
+        half = half_u = 0.0
+        if n > 1:
+            from statistics import NormalDist  # noqa: PLC0415
+            z = NormalDist().inv_cdf(0.5 + level / 2.0)
+            half = z * float(d.std(ddof=1)) / float(np.sqrt(n))
+            sa, sb = float(xa.std(ddof=1)), float(xb.std(ddof=1))
+            half_u = z * float(np.sqrt((sa * sa + sb * sb) / n))
+            if sa > 0.0 and sb > 0.0:
+                out["corr"] = float(((xa - xa.mean()) * (xb - xb.mean())).sum() / (n - 1) / (sa * sb))
+        mu = float(xa.mean()) - float(xb.mean())
+        out.update(estimate=m, lo=m - half, hi=m + half, half_width=half, unpaired=(mu, mu - half_u, mu + half_u),
+                   unpaired_half_width=half_u)
+        return out
 
     def summary(self) -> dict[str, float]:
         ok = self.completed > 0
@@ -414,6 +465,7 @@ class SweepResults:
                            self.samp_sum[index], self.samp_max[index], g(self.throughput), g(self.histograms),
                            self.replica_begin)
         out.traced = self.traced
+        out.streams = g(self.streams)
         out.band_count, out.band_sum, out.band_sumsq = self.band_count, self.band_sum, self.band_sumsq
         out.lat_window_s, out.lat_hist, out.lat_sum_hi, out.lat_sum_lo = (self.lat_window_s, self.lat_hist,
                                                                           self.lat_sum_hi, self.lat_sum_lo)
@@ -612,6 +664,8 @@ class SweepResults:
             np.concatenate([p.edge_dropped for p in parts]), np.concatenate([p.samp_sum for p in parts]),
             np.concatenate([p.samp_max for p in parts]), cat([p.throughput for p in parts]),
             cat([p.histograms for p in parts]), f.replica_begin)
+        if all(p.streams is not None for p in parts):
+            out.streams = np.concatenate([p.streams for p in parts])
         if all(p.band_count is not None for p in parts):      # integer sums over disjoint replicas: they add exactly
             out.band_count = np.sum([p.band_count for p in parts], axis=0, dtype=np.uint32)
             out.band_sum = np.sum([p.band_sum for p in parts], axis=0, dtype=np.uint64)

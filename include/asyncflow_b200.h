@@ -38,7 +38,7 @@
 extern "C" {
 #endif
 
-#define AF_ABI_VERSION 8
+#define AF_ABI_VERSION 9
 
 typedef enum AfStatus {
     AF_OK = 0,
@@ -234,6 +234,16 @@ typedef struct AfTimeline {
     const AfOutageMark* outages; /* [n_rows][n_outage_marks]                                           */
 } AfTimeline;
 int af_timeline_upload(af_engine* e, const AfTimeline* timeline, uint64_t first_replica);
+
+/* Random streams (common random numbers): replica first_replica + i, i < n, draws every random number -- users,
+ * inter-arrival gaps, edge latencies and dropouts, endpoint choices -- as if its replica id were stream_of[i]; every
+ * other replica draws as its own id, the rule sweep and timeline rows follow.  The id still picks the replica's output
+ * slot, sweep row, timeline row and band group, so two replicas with one stream see the same traffic whatever their
+ * parameters.  Any uint64_t is a stream (both words of the replica half of the Philox counter).  The table costs
+ * 8 bytes per replica on the device and is kept, across af_scenario_upload and af_sweep_upload, until the next
+ * af_streams_upload; NULL (or n = 0) clears it.  Without a table every output is the one before tables existed, and
+ * a table with stream_of[i] = first_replica + i changes no output. */
+int af_streams_upload(af_engine* e, const uint64_t* stream_of, uint64_t n, uint64_t first_replica);
 
 /* Simulate replicas [replica_begin, replica_end) start to horizon.  Asynchronous
  * on the engine's stream; af_sync / any af_fetch_* waits for it.                 */
