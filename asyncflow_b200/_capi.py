@@ -27,6 +27,10 @@ FIELDS = {
     "edge_dropout": 5, "server_cpu_cores": 6, "server_ram_mb": 7, "step_duration": 8,
     "endpoint_ram": 9, "spike_delta": 10,
 }
+#: the load balancer's sweep columns (AF_FIELD_LB_COVERED / AF_FIELD_LB_ALGORITHM): which servers it covers and its
+#: algorithm.  Kept apart from FIELDS, the scenario's numeric parameters: their values are a membership (0 / 1) and an
+#: LB_* code, and a row that changes them changes the topology (DESIGN.md §3.11).
+LB_FIELDS = {"lb_covered": 11, "lb_algorithm": 12}
 FLAG_EVENT_OVERFLOW, FLAG_REQUEST_OVERFLOW, FLAG_TRACE_TRUNCATED, FLAG_NOWQ_OVERFLOW, FLAG_LB_EMPTY = 1, 2, 4, 8, 16
 MODE_AUTO, MODE_WARP, MODE_LANE, MODE_TWO_PASS = 0, 1, 2, 3
 SELFTEST_EDGE, SELFTEST_GEN_UNIFORM, SELFTEST_GEN_USERS, SELFTEST_ENDPOINT = 0, 1, 2, 3

@@ -169,7 +169,8 @@ struct State {
     uint32_t tick_seq, n_ticks;
     double tick_time;
     // results
-    uint32_t completed, flags, traced, pad0;
+    uint32_t completed, flags, traced;
+    int32_t lb_algo;                        // the replica's AF_LB_* (its sweep row's, else the scenario's)
     uint64_t n_events;
     double lat_sum, lat_sumsq, lat_min, lat_max;
     // per-tick bands: the replica's group's difference rows (nullptr: bands off), the first tick it contributes, the
@@ -851,7 +852,7 @@ AF_FN void node_got(State& W, uint32_t node, uint32_t slot, double t0, uint32_t 
     // stops and says so (flatten() rejects timelines that can reach this state)
     if (AF_UNLIKELY(n <= 0)) { W.flags |= AF_FLAG_LB_EMPTY; return; }
     uint32_t pick = lb[0];
-    if (AF_L.lb_algo == AF_LB_ROUND_ROBIN) {         // lb_algorithms.py:22-36
+    if (W.lb_algo == AF_LB_ROUND_ROBIN) {            // lb_algorithms.py:22-36
 #pragma unroll 1
         for (int32_t i = 1; i < n; ++i) lb[i - 1] = lb[i];
         lb[n - 1] = pick;
@@ -1157,10 +1158,12 @@ AF_FN void load_params(State& W, const AfSpikeMark* spikes, const AfOutageMark* 
     for (int32_t i = lane; i < AF_L.n_servers + 2; i += WARP) { InboxS b; b.head = b.tail = NIL; b.pending = 1; b.pad = 0; tbl_inbox(W)[i] = b; }
     w_sync();
     W.users_mean = AF_L.users_mean; W.users_sigma = AF_L.users_sigma; W.rate_per_user = AF_L.rate_per_user;
+    W.lb_algo = AF_L.lb_algo;
     // sweep overrides of this replica (uniform: every lane applies every column)
     const uint64_t replica = AF_G.replica_begin + W.local;     // (W.replica is its stream)
     if (AF_L.n_sweep_cols > 0 && replica >= AF_G.sweep_first && replica - AF_G.sweep_first < AF_G.sweep_rows) {
         const double* row = AF_G.sweep_vals + (replica - AF_G.sweep_first) * (uint64_t)AF_L.n_sweep_cols;
+        bool uncovered = false;
 #pragma unroll 1
         for (int32_t c = 0; c < AF_L.n_sweep_cols; ++c) {
             const AfSweepColumn col = AF_G.sweep_cols[c];
@@ -1178,10 +1181,22 @@ AF_FN void load_params(State& W, const AfSpikeMark* spikes, const AfOutageMark* 
             case AF_FIELD_ENDPOINT_RAM: tbl_endpoint(W)[col.index].total_ram = (uint32_t)v; break;
             case AF_FIELD_SPIKE_DELTA:
                 tbl_spike(W)[col.index].delta = tbl_spike(W)[col.index].delta < 0.0 ? -v : v; break;
+            case AF_FIELD_LB_COVERED: if (v == 0.0) { tbl_lb(W)[col.index] = NIL; uncovered = true; } break;
+            case AF_FIELD_LB_ALGORITHM: W.lb_algo = (int32_t)v; break;
             default: break;
             }
         }
         w_sync();
+        if (uncovered) {                             // the LB order without the edges the row uncovers (lane 0 alone: in place)
+            if (lane == 0) {
+                uint32_t* lb = tbl_lb(W);
+                int32_t n = 0;
+#pragma unroll 1
+                for (int32_t i = 0; i < AF_L.n_lb_edges; ++i) if (lb[i] != NIL) lb[n++] = lb[i];
+                W.lb_n = n;
+            }
+            w_sync();
+        }
     }
     if (AF_G.redo_list) {                            // a re-run: the first pass left partial counts in the accumulating outputs
         if (AF_L.collect_hist) for (int32_t b = lane; b < AF_HIST_BINS; b += WARP) AF_G.hist[W.local * AF_HIST_BINS + (uint32_t)b] = 0;

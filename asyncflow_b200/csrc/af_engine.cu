@@ -380,10 +380,14 @@ struct af_engine {
     std::vector<int32_t> h_row_need;               // aflh::row_events_estimates of the sweep's rows ...
     int32_t row_need_max = 0;                      // ... and the largest of them
     DevBuf d_sweep_cols, d_sweep_vals, d_row_need;
+    // the sweep's AF_FIELD_LB_COVERED columns and their values [sweep_rows][h_cover_cols.size()] (af_run's check of the
+    // rows against the outage marks they run with; afh::lb_cover_fits)
+    std::vector<AfSweepColumn> h_cover_cols; std::vector<double> h_cover_vals;
     // per-replica timelines (af_timeline_upload): rows of replicas [tl_first, tl_first + tl_rows); the spike rows in both
     // kernels' layouts (the warp kernel reads AfSpikeMark, the lane kernel afl::SpikeP), the outage rows in the one both read
     uint64_t tl_rows = 0, tl_first = 0;
     DevBuf d_tl_spikes, d_tl_l_spikes, d_tl_outages;
+    std::vector<AfOutageMark> h_tl_outages;        // host copy of the outage rows (afh::lb_cover_fits)
     // random streams (af_streams_upload): replica stream_first + i, i < stream_rows, draws as d_streams[i]
     uint64_t stream_rows = 0, stream_first = 0;
     DevBuf d_streams;
@@ -580,6 +584,8 @@ int af_sweep_upload(af_engine* e, const AfSweep* sw, uint64_t first_replica) {
         case AF_FIELD_STEP_DURATION: lim = s.n_steps; break;
         case AF_FIELD_ENDPOINT_RAM: lim = s.n_endpoints; break;
         case AF_FIELD_SPIKE_DELTA: lim = s.n_spike_marks; break;
+        case AF_FIELD_LB_COVERED: lim = s.n_lb_edges; break;
+        case AF_FIELD_LB_ALGORITHM: lim = 1; break;
         default: return e->fail(AF_ERR_INVALID, "sweep: unknown field id");
         }
         if (i < 0 || i >= lim) return e->fail(AF_ERR_INVALID, "sweep: column index out of range");
@@ -605,6 +611,7 @@ int af_sweep_upload(af_engine* e, const AfSweep* sw, uint64_t first_replica) {
                 break;
             }
             case AF_FIELD_USERS_SIGMA: ok = ok && v >= 0.0 && s.users_dist == AF_DIST_NORMAL; break;
+            case AF_FIELD_LB_COVERED: case AF_FIELD_LB_ALGORITHM: break;      // afh::lb_sweep_fits
             default: ok = ok && v >= 0.0; break;            // users, rates, sigmas, durations, spike amplitudes
             }
             if (!ok) {
@@ -613,6 +620,10 @@ int af_sweep_upload(af_engine* e, const AfSweep* sw, uint64_t first_replica) {
                 return e->fail(AF_ERR_INVALID, b);
             }
         }
+    {
+        std::string why;
+        if (!afh::lb_sweep_fits(s, sw->columns, sw->n_columns, sw->values, sw->n_rows, why)) return e->fail(AF_ERR_INVALID, why);
+    }
     e->h_sweep_cols.assign(sw->columns, sw->columns + sw->n_columns);
     e->h_sweep_alias = aflh::column_aliases(sw->values, sw->n_rows, sw->n_columns);
     // each row's own pending-events estimate: the lane kernel splits the replica's shared-memory pool by it.  On the
@@ -628,6 +639,14 @@ int af_sweep_upload(af_engine* e, const AfSweep* sw, uint64_t first_replica) {
     AF_CUDA(e, cudaMemcpyAsync(e->d_row_need.p, e->h_row_need.data(), sw->n_rows * sizeof(int32_t), cudaMemcpyHostToDevice, e->stream),
             "sweep row estimates H2D");
     AF_CUDA(e, cudaStreamSynchronize(e->stream), "sweep upload");
+    e->h_cover_cols.clear(); e->h_cover_vals.clear();
+    for (int c = 0; c < sw->n_columns; ++c) if (sw->columns[c].field == AF_FIELD_LB_COVERED) e->h_cover_cols.push_back(sw->columns[c]);
+    if (!e->h_cover_cols.empty()) {
+        e->h_cover_vals.reserve(sw->n_rows * e->h_cover_cols.size());
+        for (uint64_t r = 0; r < sw->n_rows; ++r)
+            for (int c = 0; c < sw->n_columns; ++c)
+                if (sw->columns[c].field == AF_FIELD_LB_COVERED) e->h_cover_vals.push_back(sw->values[r * (uint64_t)sw->n_columns + (uint64_t)c]);
+    }
     e->sweep_cols = sw->n_columns; e->sweep_rows = sw->n_rows; e->sweep_first = first_replica;
     return AF_OK;
 }
@@ -652,6 +671,7 @@ int af_timeline_upload(af_engine* e, const AfTimeline* t, uint64_t first_replica
                 "timeline H2D");
     }
     if (no) AF_CUDA(e, cudaMemcpyAsync(e->d_tl_outages.p, t->outages, no * sizeof(AfOutageMark), cudaMemcpyHostToDevice, e->stream), "timeline H2D");
+    e->h_tl_outages.assign(t->outages, t->outages + no);
     AF_CUDA(e, cudaStreamSynchronize(e->stream), "timeline upload");
     e->tl_rows = t->n_rows; e->tl_first = first_replica;
     return AF_OK;
@@ -818,6 +838,13 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
     if (e->tl_rows) {
         std::string why;
         if (!afh::timeline_sweep_fits(e->h_sweep_cols.data(), e->sweep_cols, why)) return e->fail(AF_ERR_INVALID, why);
+    }
+    if (e->sweep_cols > 0 && !e->h_cover_cols.empty()) {
+        std::string why;
+        const AfTimeline tl = {e->tl_rows, nullptr, e->h_tl_outages.data()};
+        if (!afh::lb_cover_fits(e->sc, e->h_cover_cols.data(), (int32_t)e->h_cover_cols.size(), e->h_cover_vals.data(), e->sweep_first,
+                                e->sweep_rows, e->tl_rows ? &tl : nullptr, e->tl_first, begin, end, why))
+            return e->fail(AF_ERR_INVALID, why);
     }
 
     // ---- pass structure ---------------------------------------------------------------------------------

@@ -4,6 +4,7 @@
 #pragma once
 #include <math.h>
 #include <stdio.h>
+#include <algorithm>
 #include <string>
 #include <vector>
 #include "af_core.cuh"
@@ -118,6 +119,78 @@ inline bool timeline_sweep_fits(const AfSweepColumn* cols, int32_t n_cols, std::
                   "rows are uploaded; put the amplitudes in the rows' spike deltas";
             return false;
         }
+    return true;
+}
+
+// af_sweep_upload's checks of the load-balancer columns (AF_FIELD_LB_COVERED / AF_FIELD_LB_ALGORITHM): a load balancer
+// to sweep, values 0 or 1, and in every row at least one covered LB edge (two columns over one position: the later wins,
+// as in the kernels).  Index ranges are checked with the other fields'.
+inline bool lb_sweep_fits(const AfScenario& s, const AfSweepColumn* cols, int32_t n_cols, const double* vals, uint64_t n_rows,
+                          std::string& err) {
+    char buf[256];
+#define AF_CHECK(cond, ...) do { if (!(cond)) { snprintf(buf, sizeof buf, __VA_ARGS__); err = buf; return false; } } while (0)
+    bool cover = false;
+    for (int32_t c = 0; c < n_cols; ++c) {
+        const int32_t f = cols[c].field;
+        if (f != AF_FIELD_LB_COVERED && f != AF_FIELD_LB_ALGORITHM) continue;
+        AF_CHECK(s.n_lb_edges > 0 && s.lb_algo != AF_LB_NONE, "sweep: column %d sweeps the load balancer of a scenario without one", c);
+        cover = cover || f == AF_FIELD_LB_COVERED;
+        for (uint64_t r = 0; r < n_rows; ++r) {
+            const double v = vals[r * (uint64_t)n_cols + (uint64_t)c];
+            AF_CHECK(v == 0.0 || v == 1.0, "sweep: row %llu column %d (%s): value %g is neither 0 nor 1", (unsigned long long)r, c,
+                     f == AF_FIELD_LB_COVERED ? "lb_covered" : "lb_algorithm", v);
+        }
+    }
+    if (!cover) return true;
+    std::vector<char> on((size_t)s.n_lb_edges);
+    for (uint64_t r = 0; r < n_rows; ++r) {
+        std::fill(on.begin(), on.end(), (char)1);
+        for (int32_t c = 0; c < n_cols; ++c)
+            if (cols[c].field == AF_FIELD_LB_COVERED) on[(size_t)cols[c].index] = vals[r * (uint64_t)n_cols + (uint64_t)c] != 0.0;
+        bool any = false;
+        for (char x : on) any = any || x;
+        AF_CHECK(any, "sweep: row %llu covers no edge of the load balancer (AF_FIELD_LB_COVERED is 0 for all %d)",
+                 (unsigned long long)r, s.n_lb_edges);
+    }
+#undef AF_CHECK
+    return true;
+}
+
+// af_run's rule for a launch with AF_FIELD_LB_COVERED columns: no replica of [begin, end) with a sweep row (sweep row r
+// describes replica sweep_first + r) may uncover an LB edge that the outage marks it runs with still name -- its
+// timeline row (row r of `tl` describes replica tl_first + r) if it has one, else the scenario's.  Such a mark would
+// put the edge back behind the load balancer at its SERVER_UP.  `cols` / `vals` may hold the LB_COVERED columns alone.
+inline bool lb_cover_fits(const AfScenario& s, const AfSweepColumn* cols, int32_t n_cols, const double* vals,
+                          uint64_t sweep_first, uint64_t sweep_rows, const AfTimeline* tl, uint64_t tl_first,
+                          uint64_t begin, uint64_t end, std::string& err) {
+    std::vector<int32_t> cover;
+    for (int32_t c = 0; c < n_cols; ++c) if (cols[c].field == AF_FIELD_LB_COVERED) cover.push_back(c);
+    if (cover.empty() || s.n_lb_edges == 0) return true;
+    std::vector<char> on((size_t)s.n_lb_edges);
+    const uint64_t lo = begin > sweep_first ? begin : sweep_first;
+    const uint64_t hi = end < sweep_first + sweep_rows ? end : sweep_first + sweep_rows;
+    for (uint64_t id = lo; id < hi; ++id) {
+        const double* row = vals + (id - sweep_first) * (uint64_t)n_cols;
+        std::fill(on.begin(), on.end(), (char)1);
+        bool cut = false;
+        for (int32_t c : cover) { const bool v = row[c] != 0.0; on[(size_t)cols[c].index] = v; cut = cut || !v; }
+        if (!cut) continue;
+        const bool own = tl != nullptr && id - tl_first < tl->n_rows;
+        const AfOutageMark* om = own ? tl->outages + (id - tl_first) * (uint64_t)s.n_outage_marks : s.outage_marks;
+        for (int32_t i = 0; i < s.n_outage_marks; ++i) {
+            if (om[i].lb_edge < 0) continue;
+            for (int32_t k = 0; k < s.n_lb_edges; ++k)
+                if (!on[(size_t)k] && s.lb_edges[k] == om[i].lb_edge) {
+                    char b[320];
+                    snprintf(b, sizeof b, "af_run: replica %llu uncovers load-balancer edge %d (AF_FIELD_LB_COVERED position %d) "
+                             "while outage mark %d of its %s names it; give the row a timeline row whose marks of that "
+                             "server have lb_edge = -1", (unsigned long long)id, s.lb_edges[k], k, i,
+                             own ? "timeline row" : "scenario's timeline");
+                    err = b;
+                    return false;
+                }
+        }
+    }
     return true;
 }
 

@@ -202,6 +202,9 @@ struct Cfg {
     const uint64_t* stream_of;
     uint64_t stream_first, stream_rows;
 };
+// Cfg.lb_algo of a launch that sweeps the load-balancer algorithm (AF_FIELD_LB_ALGORITHM; DESIGN.md §3.11): each replica
+// reads its own from the 32-bit word right after its LB order, o32_lb + n_lb_edges
+constexpr int32_t LB_PER_REPLICA = 2;
 
 
 #if defined(__CUDACC__)
@@ -950,17 +953,29 @@ AFL_IN void start_replica(St& W, const Mem& m, uint64_t local_index) {
     // sweep overrides of this replica: fields consumed here, fields looked up during the run (row copy)
     const bool has_row = C.n_sweep_cols > 0 && W.replica >= C.sweep_first && W.replica - C.sweep_first < C.sweep_rows;
     const double* row = C.sweep_vals + (has_row ? (W.replica - C.sweep_first) * (uint64_t)C.n_sweep_cols : 0);
+    bool uncovered = false;
 #pragma unroll 1
     for (int32_t c = 0; c < C.n_sweep_cols; ++c) {
         const ColP col = C.cols[c];
         const double v = has_row ? row[c] : col.base;
         if (col.slot >= 0) { f64_st(m, C.o64_row + col.slot, v); continue; }
+        if (col.field == AF_FIELD_LB_ALGORITHM) { w32_st(m, C.o32_lb + C.n_lb_edges, (uint32_t)(int32_t)v); continue; }   // (base: the scenario's)
         if (!has_row || gen_field(col.field, v, W.users_mean, W.users_sigma, W.rate_per_user)) continue;
         switch (col.field) {
         case AF_FIELD_SERVER_CPU_CORES: i32_st(m, sv_word((uint32_t)col.index, SV_CPU_FREE), (int32_t)v); break;
         case AF_FIELD_SERVER_RAM_MB: i32_st(m, sv_word((uint32_t)col.index, SV_RAM_FREE), (int32_t)v); break;
+        case AF_FIELD_LB_COVERED: if (v == 0.0) { w32_st(m, C.o32_lb + col.index, NIL); uncovered = true; } break;
         default: break;
         }
+    }
+    if (uncovered) {                                  // the LB order without the edges the row uncovers
+        int32_t n = 0;
+#pragma unroll 1
+        for (int32_t i = 0; i < C.n_lb_edges; ++i) {
+            const uint32_t e = w32_ld(m, C.o32_lb + i);
+            if (e != NIL) w32_st(m, C.o32_lb + n++, e);
+        }
+        W.lb_n = n;
     }
     if (C.redo) {                                     // a re-run: the first pass left partial counts in the accumulating outputs
         if (C.collect_hist) for (int32_t b = 0; b < AF_HIST_BINS; ++b) C.hist[W.local * AF_HIST_BINS + (uint32_t)b] = 0;
@@ -1293,7 +1308,9 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                     if (AFL_UNLIKELY(n <= 0)) { rq_pack_set(W, m, slot, pack); W.flags |= AF_FLAG_LB_EMPTY; }
                     else {
                         uint32_t pick = w32_ld(m, lb);
-                        if (C.lb_algo == AF_LB_ROUND_ROBIN) {      // lb_algorithms.py:22-36
+                        // (a launch that sweeps the algorithm keeps each replica's next to its LB order)
+                        if (C.lb_algo == AF_LB_ROUND_ROBIN
+                            || (C.lb_algo == LB_PER_REPLICA && w32_ld(m, lb + C.n_lb_edges) == (uint32_t)AF_LB_ROUND_ROBIN)) {   // lb_algorithms.py:22-36
 #pragma unroll 1
                             for (int32_t i = 1; i < n; ++i) w32_st(m, lb + i - 1, w32_ld(m, lb + i));
                             w32_st(m, lb + n - 1, pick);

@@ -14,12 +14,13 @@ struct Tables {
     std::vector<afl::StepP> steps; std::vector<afl::SpikeP> spikes; std::vector<afl::OutageP> outages;
     std::vector<int32_t> lb; std::vector<afl::ColP> cols;
     int32_t n_row = 0;
+    int32_t lb_algo_word = 0;      // 1: a column sweeps the LB algorithm (a 32-bit word per lane after the LB order)
 };
 
 // Scenario (+ the sweep's columns) -> the kernel's read-only tables.  A column over a field the kernel
 // looks up during the run (edge latency parameters, step durations, endpoint RAM, spike amplitudes) gets a
-// slot in the lane's row copy; a column over a field consumed at the start of a replica (users, cores, RAM)
-// does not.  Two columns over the same (field, index): the later one wins, as in af_core.cuh::load_params.
+// slot in the lane's row copy; a column over a field consumed at the start of a replica (users, cores, RAM, the LB's
+// pool and algorithm) does not.  Two columns over the same (field, index): the later one wins, as in af_core.cuh::load_params.
 inline bool build_tables(const AfScenario& s, const AfSweepColumn* cols, int32_t n_cols, const int32_t* alias, Tables& t, std::string& err) {
     t = Tables();
     t.edges.resize((size_t)s.n_edges);
@@ -73,6 +74,8 @@ inline bool build_tables(const AfScenario& s, const AfSweepColumn* cols, int32_t
         case AF_FIELD_ENDPOINT_RAM: k.slot = AFLH_SLOT(); k.base = s.endpoints[i].total_ram; t.endpoints[(size_t)i].c_ram = k.slot; break;
         case AF_FIELD_SPIKE_DELTA: k.slot = AFLH_SLOT(); k.base = s.spike_marks[i].delta < 0.0 ? -s.spike_marks[i].delta : s.spike_marks[i].delta;
                                    t.spikes[(size_t)i].c_delta = k.slot; break;
+        case AF_FIELD_LB_COVERED: k.base = 1.0; break;
+        case AF_FIELD_LB_ALGORITHM: k.base = s.lb_algo; t.lb_algo_word = 1; break;
         default: err = "sweep: unknown field id"; return false;
         }
 #undef AFLH_SLOT
@@ -193,7 +196,7 @@ constexpr int32_t LANE_REQUEST_CAPACITY = 2048;
 inline int32_t fixed_lane_bytes(const AfScenario& s, const Tables& t) {
     const int32_t n_series = 3 * s.n_servers + s.n_edges;
     const int32_t fix64 = (s.n_spike_marks > 0 ? s.n_edges : 0) + t.n_row;
-    const int32_t fix32 = s.n_edges + afl::SV_WORDS * s.n_servers + s.n_lb_edges + (n_series + 31) / 32;
+    const int32_t fix32 = s.n_edges + afl::SV_WORDS * s.n_servers + s.n_lb_edges + t.lb_algo_word + (n_series + 31) / 32;
     return 8 * fix64 + 4 * fix32;
 }
 constexpr int32_t MIN_DYNAMIC_BYTES = 16 * 4 + 36 * 2;      // (a pool of 8 elements: 4 heap entries, 2 records and more)
@@ -227,7 +230,7 @@ inline bool lean_launch(const AfScenario& s, int32_t trace_replicas) {
 // (afl::LANES is a property of the compilation pass, and the host pass of a .cu file sees 1).
 inline bool make_cfg(const AfScenario& s, const AfOptions& o, const Tables& t, int32_t lane_bytes, int32_t trace_tick_cap, int32_t lanes, afl::Cfg& C, int32_t ev_need = 0, int32_t rq_min = 2) {
     C.n_edges = s.n_edges; C.n_servers = s.n_servers; C.n_endpoints = s.n_endpoints; C.n_steps = s.n_steps;
-    C.n_lb_edges = s.n_lb_edges; C.lb_algo = s.lb_algo; C.gen_edge = s.gen_edge; C.client_edge = s.client_edge;
+    C.n_lb_edges = s.n_lb_edges; C.lb_algo = t.lb_algo_word ? afl::LB_PER_REPLICA : s.lb_algo; C.gen_edge = s.gen_edge; C.client_edge = s.client_edge;
     C.n_spike = s.n_spike_marks; C.n_outage = s.n_outage_marks;
     C.users_dist = s.users_dist; C.window_s = s.window_s; C.horizon_s = s.horizon_s; C.metrics_mask = s.metrics_mask;
     C.users_mean = s.users_mean; C.users_sigma = s.users_sigma; C.rate_per_user = s.rate_per_user; C.sample_period = s.sample_period;
@@ -242,7 +245,7 @@ inline bool make_cfg(const AfScenario& s, const AfOptions& o, const Tables& t, i
     // fixed part of a lane's shared memory
     const int32_t fix64 = (C.n_spike > 0 ? C.n_edges : 0) + C.n_row;
     C.n_dirty = (C.n_series + 31) / 32;
-    const int32_t fix32 = C.n_edges + afl::SV_WORDS * C.n_servers + C.n_lb_edges + C.n_dirty;
+    const int32_t fix32 = C.n_edges + afl::SV_WORDS * C.n_servers + C.n_lb_edges + t.lb_algo_word + C.n_dirty;
     int32_t nq_s = 0;                                // zero-delay items: ties only -- the ring starts in the global tier
     const int32_t rest = lane_bytes - 8 * fix64 - 4 * fix32;
     // the rest is the pool: 16-byte elements shared by the heap and the request records, split per replica
@@ -271,7 +274,7 @@ inline bool make_cfg(const AfScenario& s, const AfOptions& o, const Tables& t, i
     int32_t w = 0;
     C.o32_conn = w; w += C.n_edges;
     C.o32_srv = w; w += afl::SV_WORDS * C.n_servers;
-    C.o32_lb = w; w += C.n_lb_edges;
+    C.o32_lb = w; w += C.n_lb_edges + t.lb_algo_word;
     C.o32_dirty = w; w += C.n_dirty;
     C.n32 = w;
     C.warp_bytes = (C.n128 * 16 + C.n64 * 8 + C.n32 * 4) * lanes;

@@ -61,6 +61,19 @@ OUTAGE_MARK_DTYPE = np.dtype([("fire_time", "<f8"), ("lb_edge", "<i4"), ("down",
 assert SPIKE_MARK_DTYPE.itemsize == C.sizeof(K.AfSpikeMark) and OUTAGE_MARK_DTYPE.itemsize == C.sizeof(K.AfOutageMark)
 
 
+#: ``lb_algorithm`` sweep values: ``K.LB_*`` code -> the reference's name (routing/lb_algorithms.py)
+LB_ALGORITHMS = {K.LB_ROUND_ROBIN: "round_robin", K.LB_LEAST_CONNECTIONS: "least_connection"}
+
+
+def _lb_position(flat: "FlatScenario", server_id: str) -> int:
+    """Position in ``flat.lb_edges`` of the load balancer's edge to ``server_id`` (``KeyError`` when it covers none)."""
+    for k, e in enumerate(flat.lb_edges):
+        if flat.server_ids[flat.pod.edges[e].target_index] == server_id:
+            return k
+    msg = f"sweep column ('lb_covered', {server_id!r}): the scenario's load balancer does not cover that server"
+    raise KeyError(msg)
+
+
 def _rv(d: dict) -> tuple[str, float, float]:
     dist = _s(d.get("distribution") or "poisson")
     var = d.get("variance")
@@ -153,10 +166,13 @@ def _sorted_fold(events: list[FlatEvent], t_start: np.ndarray, t_end: np.ndarray
 
 
 def build_timelines(events: list[FlatEvent], lb_edges: list[int], horizon: float, t_start: np.ndarray,
-                    t_end: np.ndarray, spike_s: np.ndarray, label=lambda r: "") -> Timelines:
+                    t_end: np.ndarray, spike_s: np.ndarray, label=lambda r: "", covered: np.ndarray | None = None) -> Timelines:
     """The spike and outage mark tables of R rows of event times (``t_start`` / ``t_end`` / ``spike_s``: [R, n_events],
     columns in the order of ``events``): what ``flatten`` uploads for one row and ``SweepSpec`` for each of its rows.
-    Refuses (``ValueError``, prefixed by ``label(row)``) a row whose load balancer runs out of servers before the horizon."""
+    ``covered`` ([R, len(lb_edges)] bool, default all): which LB edges each row keeps; an outage mark of a server whose
+    edge a row leaves out gets ``lb_edge = -1`` there (the reference's no-op for a server not behind the LB), its fire
+    time unchanged.  Refuses (``ValueError``, prefixed by ``label(row)``) a row whose load balancer runs out of servers
+    before the horizon."""
     sp = [i for i, e in enumerate(events) if e.spike]
     out = [i for i, e in enumerate(events) if not e.spike]
     R = t_start.shape[0]
@@ -178,8 +194,15 @@ def build_timelines(events: list[FlatEvent], lb_edges: list[int], horizon: float
     if lb_edges and out:                                # replay of the outage marks over the LB's edge set
         pos = np.zeros(max(lb_edges) + 1, dtype=np.int64)      # LB edge -> its column of `up`
         pos[lb_edges] = np.arange(len(lb_edges))
-        up = np.ones((R, len(lb_edges)), dtype=bool)
+        up = np.ones((R, len(lb_edges)), dtype=bool) if covered is None else np.array(covered, dtype=bool)
         rows = np.arange(R)
+        if covered is not None:
+            for j in range(o_mark.shape[1]):
+                le = outages["lb_edge"][:, j]
+                hit = le >= 0
+                cut = np.zeros(R, dtype=bool)
+                cut[hit] = ~up[rows[hit], pos[le[hit]]]
+                outages["lb_edge"][cut, j] = -1
         for j in range(o_mark.shape[1]):
             le, down = outages["lb_edge"][:, j], outages["down"][:, j] != 0
             hit = le >= 0
@@ -389,7 +412,15 @@ class SweepSpec:
     ``("server_cpu_cores"|"server_ram_mb", server_id)``,
     ``("step_duration", server_id, endpoint_idx, step_idx)``,
     ``("endpoint_ram", server_id, endpoint_idx)``, ``("spike_delta", event_id)``,
-    ``("event_start"|"event_end", event_id)`` (the ``t_start`` / ``t_end`` of a spike or an outage).
+    ``("event_start"|"event_end", event_id)`` (the ``t_start`` / ``t_end`` of a spike or an outage),
+    ``("lb_covered", server_id)`` (1: behind the load balancer as in the scenario, 0: not; bools accepted) and
+    ``("lb_algorithm",)`` (``"round_robin"`` or ``"least_connection"``, enum members or ``K.LB_*`` codes accepted).
+
+    A row that uncovers a server simulates the scenario without the load balancer's edge to it (:meth:`payload_for`):
+    its round-robin order is the scenario's with that edge left out, and an outage of that server is a no-op.  The
+    scenario's load balancer covers the largest fleet: only servers it covers can be swept.  A row that covers no
+    server, uncovers a server whose LB edge a spike targets, or whose covered servers are all down at once is refused
+    with a ``ValueError`` naming the row.
 
     A spec that sweeps an event time gives every row its own spike and outage timelines (:attr:`timelines`, uploaded
     with the sweep): the marks sorted and their fire times folded as ``flatten`` does for the scenario, a row's
@@ -406,11 +437,17 @@ class SweepSpec:
         cols: list[tuple[int, int]] = []
         vals: list[np.ndarray] = []
         keys = [tuple(sel) if not isinstance(sel, str) else (sel,) for sel in columns]
-        times = any(k[0] in ("event_start", "event_end") for k in keys)
+        arrays = [self._lb_values(flat, sel, v) if sel[0] in ("lb_covered", "lb_algorithm")
+                  else np.ascontiguousarray(np.broadcast_to(np.asarray(v, dtype=np.float64), (self.n_replicas,)))
+                  for sel, v in zip(keys, columns.values())]
+        self.covered = self._covered(flat, keys, arrays)
+        # rows need their own timelines when event times are swept or when a row drops a server that has outage marks
+        times = any(k[0] in ("event_start", "event_end") for k in keys) or (
+            self.covered is not None and any((~self.covered[:, flat.lb_edges.index(e.target)]).any()
+                                             for e in flat.events if not e.spike and e.target >= 0))
         event_of = {e.event_id: i for i, e in enumerate(flat.events)}
-        for sel, v in zip(keys, columns.values()):
+        for sel, arr in zip(keys, arrays):
             name = sel[0]
-            arr = np.ascontiguousarray(np.broadcast_to(np.asarray(v, dtype=np.float64), (self.n_replicas,)))
             if name in ("event_start", "event_end") or (times and name == "spike_delta"):
                 if sel[1] not in event_of or (name == "spike_delta" and not flat.events[event_of[sel[1]]].spike):
                     msg = f"no {'spike ' if name == 'spike_delta' else ''}event {sel[1]!r}"
@@ -432,12 +469,16 @@ class SweepSpec:
                 if not targets:
                     msg = f"no spike event {sel[1]!r}"
                     raise KeyError(msg)
+            elif name == "lb_covered":
+                targets = [_lb_position(flat, sel[1])]
+            elif name == "lb_algorithm":
+                targets = [0]
             else:
                 msg = f"unknown sweep field {name!r}"
                 raise KeyError(msg)
             self.selectors.append((sel, arr))
             for t in targets:
-                cols.append((K.FIELDS[name], t))
+                cols.append(((K.LB_FIELDS if name in K.LB_FIELDS else K.FIELDS)[name], t))
                 vals.append(arr)
         self.n_columns = len(cols)
         self.values = (np.ascontiguousarray(np.stack(vals, axis=1)) if vals
@@ -446,6 +487,65 @@ class SweepSpec:
         self.columns = cols
         if times:
             self.timelines = self._timelines(flat)
+        elif self.covered is not None and any(not e.spike for e in flat.events):
+            self._timelines(flat)               # the fleet-down check alone: every row runs the scenario's marks
+
+    def _lb_values(self, flat: FlatScenario, sel: tuple, v: Any) -> np.ndarray:
+        """A load-balancer column as float codes: 0 / 1 for ``lb_covered``, ``K.LB_*`` for ``lb_algorithm``."""
+        if flat.lb_id is None:
+            msg = f"sweep column {sel!r}: the scenario has no load balancer to sweep"
+            raise ValueError(msg)
+        raw = np.broadcast_to(np.asarray(v, dtype=object), (self.n_replicas,))
+        if sel[0] == "lb_algorithm":
+            code = {name: float(c) for c, name in LB_ALGORITHMS.items()}
+
+            def one(x: Any) -> float:
+                if isinstance(x, (int, float, np.integer, np.floating)) and not isinstance(x, (bool, np.bool_)):
+                    return float(x) if x in LB_ALGORITHMS else np.nan
+                return code.get(_s(x), np.nan)
+            out = np.array([one(x) for x in raw], dtype=np.float64)
+            bad = np.isnan(out)
+            if bad.any():
+                r = int(np.flatnonzero(bad)[0])
+                msg = (f"sweep row {r}: {sel!r} = {raw[r]!r}: the algorithm is 'round_robin' or 'least_connection' "
+                       "(or K.LB_ROUND_ROBIN / K.LB_LEAST_CONNECTIONS)")
+                raise ValueError(msg)
+            return out
+        try:
+            out = np.asarray(raw.astype(np.float64))
+        except (TypeError, ValueError):
+            out = np.full(self.n_replicas, np.nan)
+        bad = ~((out == 0.0) | (out == 1.0))
+        if bad.any():
+            r = int(np.flatnonzero(bad)[0])
+            msg = f"sweep row {r}: {sel!r} = {raw[r]!r}: a server is covered (1) or not (0)"
+            raise ValueError(msg)
+        return np.ascontiguousarray(out)
+
+    def _covered(self, flat: FlatScenario, keys: list[tuple], arrays: list[np.ndarray]) -> np.ndarray | None:
+        """[R, len(flat.lb_edges)] bool: the LB edges each row keeps (``None`` without ``lb_covered`` columns), checked
+        against the rules that need no timeline: a covered server in every row, no uncovered edge a spike targets."""
+        sel_arr = [(sel, arr) for sel, arr in zip(keys, arrays) if sel[0] == "lb_covered"]
+        if not sel_arr:
+            return None
+        cov = np.ones((self.n_replicas, len(flat.lb_edges)), dtype=bool)
+        for sel, arr in sel_arr:
+            cov[:, _lb_position(flat, sel[1])] = arr != 0.0
+        none = ~cov.any(axis=1)
+        if none.any():
+            r = int(np.flatnonzero(none)[0])
+            msg = f"sweep row {r}: ('lb_covered', ...): the row covers no server; the load balancer needs one"
+            raise ValueError(msg)
+        for e in flat.events:
+            if e.spike and e.target in flat.lb_edges:
+                k = flat.lb_edges.index(e.target)
+                if not cov[:, k].all():
+                    r = int(np.flatnonzero(~cov[:, k])[0])
+                    msg = (f"sweep row {r}: ('lb_covered', {flat.server_ids[flat.pod.edges[e.target].target_index]!r}) = 0: "
+                           f"the spike {e.event_id!r} targets the load balancer's edge to that server; a server whose LB "
+                           "edge is spiked cannot be uncovered")
+                    raise ValueError(msg)
+        return cov
 
     def _timelines(self, flat: FlatScenario) -> Timelines:
         """Every row's event times and amplitudes, checked against the payload rules, then its mark tables."""
@@ -490,7 +590,7 @@ class SweepSpec:
                     down &= np.any([(ts[:, e] <= t) & (t < te[:, e]) for e in evs], axis=0)
                 if down.any():
                     refuse(down, e0, "every server is down once it starts; keep at least one up")
-        return build_timelines(ev, flat.lb_edges, H, ts, te, amp, label=lambda r: f"sweep row {r}: ")
+        return build_timelines(ev, flat.lb_edges, H, ts, te, amp, label=lambda r: f"sweep row {r}: ", covered=self.covered)
 
     def timeline_pod(self, first: int = 0, count: int | None = None) -> tuple[K.AfTimeline | None, Any]:
         """AfTimeline over rows ``[first, first+count)`` (``None`` when the spec sweeps no event time); keep the returned
@@ -539,6 +639,7 @@ class SweepSpec:
         topo = p["topology_graph"]
         edges = {e["id"]: e for e in topo["edges"]}
         servers = {s["id"]: s for s in topo["nodes"]["servers"]}
+        uncovered: set[str] = set()
         # endpoint_ram rewrites the step list, so it goes last (step selectors use original indices)
         for sel, arr in sorted(self.selectors, key=lambda sa: sa[0][0] == "endpoint_ram"):
             name, v = sel[0], float(arr[replica])
@@ -579,6 +680,17 @@ class SweepSpec:
                             ev["start"]["t_start"] = v
                         else:
                             ev["end"]["t_end"] = v
+            elif name == "lb_covered":
+                if v == 0.0:
+                    uncovered.add(sel[1])
+                else:
+                    uncovered.discard(sel[1])
+            elif name == "lb_algorithm":
+                topo["nodes"]["load_balancer"]["algorithms"] = LB_ALGORITHMS[int(v)]
+        if uncovered:           # the reduced payload: the server stays, the LB neither covers it nor has an edge to it
+            lb = topo["nodes"]["load_balancer"]
+            lb["server_covered"] = [sid for sid in lb.get("server_covered") or [] if sid not in uncovered]
+            topo["edges"] = [e for e in topo["edges"] if not (e["source"] == lb["id"] and e["target"] in uncovered)]
         return p
 
     def pin(self) -> None:

@@ -148,8 +148,17 @@ enum {
     AF_FIELD_SERVER_CPU_CORES = 6, AF_FIELD_SERVER_RAM_MB = 7,
     AF_FIELD_STEP_DURATION = 8, AF_FIELD_ENDPOINT_RAM = 9,
     AF_FIELD_SPIKE_DELTA = 10,   /* index = spike mark; sign is kept by the engine */
-    AF_FIELD_COUNT = 11
+    AF_FIELD_LB_COVERED = 11,    /* index = position in lb_edges; 1 = behind the LB as in the scenario, 0 = not */
+    AF_FIELD_LB_ALGORITHM = 12,  /* index 0; an AF_LB_* algorithm (round robin or least connections)           */
+    AF_FIELD_COUNT = 13
 };
+/* Load-balancer rows (DESIGN.md §3.11).  A replica whose row sets AF_FIELD_LB_COVERED of position k to 0 runs without
+ * the LB edge lb_edges[k]: its round-robin order is lb_edges with the uncovered edges left out; the server and its other
+ * edges stay.  AF_FIELD_LB_ALGORITHM picks the replica's algorithm.  Replicas without a row keep the scenario's pool
+ * and algorithm.  af_sweep_upload refuses (AF_ERR_INVALID) either field on a scenario without a load balancer, an index
+ * out of range, a value other than 0 or 1, and a row that covers no edge (naming the row).  af_run refuses a launch in
+ * which a row uncovers an LB edge that the outage marks it runs with (its timeline row, else the scenario's) still name:
+ * give such rows timeline rows whose marks for that server have lb_edge = -1. */
 typedef struct AfSweepColumn { int32_t field; int32_t index; } AfSweepColumn;
 typedef struct AfSweep {
     int32_t n_columns;
