@@ -134,7 +134,10 @@ struct ServerS {          // 64 B
     uint32_t ramq_head, ramq_tail, cpuq_head, cpuq_tail;
     uint32_t out_edge, ep_begin, n_ep;
     uint32_t ramq_head_need;   // total_ram of the request at the head of the RAM queue (valid when ramq_head != NIL)
-    uint32_t pad[3];
+    // admission limit (DESIGN.md §3.12): admissions left before the server sheds (0xFFFFFFFF: no limit; one per request
+    // in service), requests shed
+    uint32_t adm_left, rejected;
+    uint32_t pad;
 };
 struct EndpointS { uint32_t step_begin, n_steps, total_ram, pad; }; // 16 B
 struct StepS { double dur; uint32_t kind, pad; };                   // 16 B
@@ -228,6 +231,9 @@ struct BandArgs {
     uint32_t dist_bins, dist_pad;
     // occupancy integrals (occ == nullptr: off): [n_replicas][5 n_servers + n_edges] u64, occ_scale = 2^f
     uint64_t* occ; double occ_scale;
+    // requests each server shed at its admission limit (nullptr: the launch has no limit; DESIGN.md §3.12):
+    // [n_replicas][n_servers] u32, written with the replica's other outputs
+    uint32_t* server_rejected;
 };
 
 // Per-replica timelines of a launch (af_sim_kernel's parameter; rows == 0: none): replica first + r, r < rows, copies its
@@ -735,6 +741,7 @@ AF_FN void run_steps(State& W, uint32_t slot, uint32_t sidx, uint32_t rid, uint3
             if (!can_fuse(W)) { nq_push(W, I_RAM_PUT, sidx, slot); return; }
             if (AF_UNLIKELY(S.ramq_head != NIL)) ram_walk(W, S, sidx);   // the put event would run next: waiters, then forward
         }
+        S.adm_left += 1;                             // out of service: handed to the out-edge
         edge_send(W, slot, S.out_edge, rid, pk_hops(pack));
         return;
     }
@@ -753,6 +760,12 @@ AF_IN void on_cpu_put(State& W, uint32_t slot, uint32_t sidx) {
 AF_IN void server_got(State& W, uint32_t slot, uint32_t sidx, const ReqRec& r) {
     consumer_get(W, NODE_SERVER0 + sidx);            // the dispatcher loops back to get() first
     ServerS& S = tbl_server(W)[sidx];
+    if (AF_UNLIKELY(S.adm_left == 0)) {              // at its admission limit: shed at the door, no handler
+        S.rejected += 1;
+        rq_release(W, slot);
+        return;
+    }
+    S.adm_left -= 1;
     uint32_t pack = r.pack + 1;                      // record_hop(SERVER)
     uint32_t epi = 0;
     const uint32_t n_ep = S.n_ep;
@@ -899,6 +912,7 @@ AF_IN void run_item(State& W, uint32_t item) {
         ServerS& S = tbl_server(W)[aux];
         ram_walk(W, S, aux);
         ReqRec r = rq_load(W, slot);
+        S.adm_left += 1;
         edge_send(W, slot, S.out_edge, r.rid, pk_hops(r.pack));
     }
 }
@@ -1121,7 +1135,7 @@ AF_FN void load_params(State& W, const AfSpikeMark* spikes, const AfOutageMark* 
         s.cpu_free = a.cpu_cores; s.ram_free = a.ram_mb; s.ready_q = 0; s.io_q = 0; s.ram_in_use = 0;
         s.ramq_head = s.ramq_tail = s.cpuq_head = s.cpuq_tail = NIL;
         s.out_edge = (uint32_t)a.out_edge; s.ep_begin = (uint32_t)a.endpoint_begin; s.n_ep = (uint32_t)a.n_endpoints;
-        s.ramq_head_need = 0; s.pad[0] = s.pad[1] = s.pad[2] = 0;
+        s.ramq_head_need = 0; s.adm_left = a.max_in_service > 0 ? (uint32_t)a.max_in_service : 0xFFFFFFFFu; s.rejected = 0; s.pad = 0;
         tbl_server(W)[i] = s;
     }
 #pragma unroll 1
@@ -1183,6 +1197,7 @@ AF_FN void load_params(State& W, const AfSpikeMark* spikes, const AfOutageMark* 
                 tbl_spike(W)[col.index].delta = tbl_spike(W)[col.index].delta < 0.0 ? -v : v; break;
             case AF_FIELD_LB_COVERED: if (v == 0.0) { tbl_lb(W)[col.index] = NIL; uncovered = true; } break;
             case AF_FIELD_LB_ALGORITHM: W.lb_algo = (int32_t)v; break;
+            case AF_FIELD_SERVER_MAX_IN_SERVICE: tbl_server(W)[col.index].adm_left = v > 0.0 ? (uint32_t)v : 0xFFFFFFFFu; break;
             default: break;
             }
         }
@@ -1343,6 +1358,11 @@ AF_IN void run_replica(State& W, uint64_t local_index, const BandArgs& band, con
     if ((W.band != nullptr || W.dist != nullptr) && (W.flags & STOP_FLAGS)) band_stop(W);   // before the frozen ticks to the horizon
     take_samples(W, W.horizon, 0u);                   // ticks strictly before the horizon
     write_back(W);
+    if (band.server_rejected != nullptr) {
+        for (int32_t i = lane_id(); i < AF_L.n_servers; i += WARP)
+            band.server_rejected[local_index * (uint64_t)AF_L.n_servers + (uint32_t)i] = tbl_server(W)[i].rejected;
+        w_sync();
+    }
 }
 AF_IN void run_replica(State& W, uint64_t local_index, const BandArgs& band, const TimelineArgs& tl) {
     const StreamArgs none = {};

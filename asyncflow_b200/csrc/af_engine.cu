@@ -428,6 +428,9 @@ struct af_engine {
     // af_occupancy_configure: on / off and f; the [n][occ_cols] rows of the last run
     AfOccupancyOptions occ_opt{0, 32};
     DevBuf d_occ;
+    // requests shed at admission limits, [n][n_servers] (DESIGN.md §3.12); written by launches with a limit somewhere
+    DevBuf d_rejected;
+    bool last_adm = false;
     bool last_occ = false; int32_t last_occ_bits = 0, last_occ_cols = 0;
 
     int fail(int code, const std::string& m) { err = m; return code; }
@@ -580,7 +583,7 @@ int af_sweep_upload(af_engine* e, const AfSweep* sw, uint64_t first_replica) {
         switch (f) {
         case AF_FIELD_USERS_MEAN: case AF_FIELD_USERS_SIGMA: case AF_FIELD_RATE_PER_USER: lim = 1; break;
         case AF_FIELD_EDGE_MEAN: case AF_FIELD_EDGE_SIGMA: case AF_FIELD_EDGE_DROPOUT: lim = s.n_edges; break;
-        case AF_FIELD_SERVER_CPU_CORES: case AF_FIELD_SERVER_RAM_MB: lim = s.n_servers; break;
+        case AF_FIELD_SERVER_CPU_CORES: case AF_FIELD_SERVER_RAM_MB: case AF_FIELD_SERVER_MAX_IN_SERVICE: lim = s.n_servers; break;
         case AF_FIELD_STEP_DURATION: lim = s.n_steps; break;
         case AF_FIELD_ENDPOINT_RAM: lim = s.n_endpoints; break;
         case AF_FIELD_SPIKE_DELTA: lim = s.n_spike_marks; break;
@@ -599,6 +602,7 @@ int af_sweep_upload(af_engine* e, const AfSweep* sw, uint64_t first_replica) {
             case AF_FIELD_EDGE_DROPOUT: ok = ok && v >= 0.0 && v <= 1.0; break;
             case AF_FIELD_SERVER_CPU_CORES: case AF_FIELD_SERVER_RAM_MB: ok = ok && v >= 1.0 && v <= 2147483647.0; break;
             case AF_FIELD_ENDPOINT_RAM: ok = ok && v >= 0.0 && v <= 2147483647.0; break;
+            case AF_FIELD_SERVER_MAX_IN_SERVICE: break;                         // afh::admission_sweep_fits
             case AF_FIELD_EDGE_MEAN: {
                 const int d = s.edges[sw->columns[c].index].dist;
                 ok = ok && (v >= 0.0 || d == AF_DIST_LOG_NORMAL || d == AF_DIST_NORMAL);
@@ -622,7 +626,8 @@ int af_sweep_upload(af_engine* e, const AfSweep* sw, uint64_t first_replica) {
         }
     {
         std::string why;
-        if (!afh::lb_sweep_fits(s, sw->columns, sw->n_columns, sw->values, sw->n_rows, why)) return e->fail(AF_ERR_INVALID, why);
+        if (!afh::lb_sweep_fits(s, sw->columns, sw->n_columns, sw->values, sw->n_rows, why)
+            || !afh::admission_sweep_fits(sw->columns, sw->n_columns, sw->values, sw->n_rows, why)) return e->fail(AF_ERR_INVALID, why);
     }
     e->h_sweep_cols.assign(sw->columns, sw->columns + sw->n_columns);
     e->h_sweep_alias = aflh::column_aliases(sw->values, sw->n_rows, sw->n_columns);
@@ -980,7 +985,8 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
     uint64_t lgrid = 0; size_t lsmem = 0;
     // the lean build of the loop when the launch cannot reach what it leaves out; ASYNCFLOW_B200_LANE_FULL (A/B
     // experiments) keeps the full one
-    const bool lean = lane && aflh::lean_launch(e->sc, o.trace_replicas) && getenv("ASYNCFLOW_B200_LANE_FULL") == nullptr;
+    const bool lean = lane && aflh::lean_launch(e->sc, o.trace_replicas, e->h_sweep_cols.data(), e->sweep_cols)
+                      && getenv("ASYNCFLOW_B200_LANE_FULL") == nullptr;
     void (*const lane_kernel)() = bands ? (lat ? lane_kernel_for<true, true>(lean, dist, occ) : lane_kernel_for<true, false>(lean, dist, occ))
                                         : (lat ? lane_kernel_for<false, true>(lean, dist, occ) : lane_kernel_for<false, false>(lean, dist, occ));
     if (lane) {
@@ -1040,6 +1046,8 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
         AF_CUDA(e, e->d_lat_from.ensure(n * 4), "latency band completions");
     }
     if (occ) AF_CUDA(e, e->d_occ.ensure(n * (uint64_t)occ_cols * 8), "occupancy rows");
+    const bool adm = afh::admission_launch(e->sc, e->h_sweep_cols.data(), e->sweep_cols);
+    if (adm) AF_CUDA(e, e->d_rejected.ensure(n * (uint64_t)L.n_servers * 4), "rejection counts");
     // pull order: the first pass runs `workers` replicas at once (lanes, or warps without the thread-per-replica pass)
     const uint64_t workers = lane ? lgrid * (uint64_t)lane_warps * 32ull : warp_slots;
     const uint64_t wave = workers < n ? workers : n;
@@ -1083,6 +1091,7 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
     G.redo_list = redo ? (const uint32_t*)e->d_redo_list.p : nullptr;
     G.redo_count = redo ? (const uint32_t*)e->d_redo_count.p : nullptr;
     G.seed = seed; G.replica_begin = begin; G.n_replicas = n;
+    band.server_rejected = adm ? (uint32_t*)e->d_rejected.p : nullptr;
     if (occ) { band.occ = (uint64_t*)e->d_occ.p; band.occ_scale = ldexp(1.0, e->occ_opt.frac_bits); }
     afc::TimelineArgs tl = {};
     if (e->tl_rows) {
@@ -1140,6 +1149,7 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
             C.tl_first = e->tl_first; C.tl_rows = e->tl_rows;
         }
         C.stream_of = rs.stream_of; C.stream_first = rs.first; C.stream_rows = rs.rows;
+        C.server_rejected = band.server_rejected;
     }
 
     // ---- enqueue ---------------------------------------------------------------------------------------------------
@@ -1158,6 +1168,7 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
     if (bands) AF_CUDA(e, cudaMemsetAsync(e->d_band.p, 0, band_words * 8, e->stream), "memset band rows");
     if (lat) AF_CUDA(e, cudaMemsetAsync(e->d_lat.p, 0, lat_words * 8, e->stream), "memset latency band rows");
     if (dist) AF_CUDA(e, cudaMemsetAsync(e->d_dist.p, 0, dist_words * 4, e->stream), "memset distribution band rows");
+    if (adm) AF_CUDA(e, cudaMemsetAsync(e->d_rejected.p, 0, n * (uint64_t)L.n_servers * 4, e->stream), "memset rejection counts");
     {   // the pull order: (work, local index) heaviest first; then the first wave grouped by estimate
         uint32_t* key = (uint32_t*)e->d_okey.p; uint32_t* idx = (uint32_t*)e->d_oidx.p; uint32_t* order = (uint32_t*)e->d_order.p;
         uint64_t* key64 = (uint64_t*)e->d_okey64.p;
@@ -1214,7 +1225,7 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
         e->launches += 1;
     }
     AF_CUDA(e, cudaEventRecord(e->ev_end, e->stream), "event");
-    e->last_n = n; e->ran = true; e->timing_valid = false;
+    e->last_n = n; e->ran = true; e->timing_valid = false; e->last_adm = adm;
     e->last_lane = lane; e->last_warp = warp; e->last_lean = lean; e->last_lane_warps = lane_warps;
     e->last_bands = bands; e->last_band_groups = e->band_groups; e->last_band_ticks = (uint32_t)band_ticks;
     e->last_band_stride = band_stride;
@@ -1317,6 +1328,13 @@ int af_fetch_edge_counts(af_engine* e, uint32_t* sent, uint32_t* dropped, uint64
     int rc = fetch(e, sent, e->d_sent, n * e->L.n_edges * 4, n, "edge sent D2H");
     if (rc) return rc;
     return fetch(e, dropped, e->d_dropped, n * e->L.n_edges * 4, n, "edge dropped D2H");
+}
+int af_fetch_server_rejected(af_engine* e, uint32_t* out, uint64_t n) {
+    if (e && e->ran && out && n == e->last_n && !e->last_adm) {      // no limit anywhere: nothing was shed
+        memset(out, 0, n * (uint64_t)e->L.n_servers * 4);
+        return AF_OK;
+    }
+    return fetch(e, out, e->d_rejected, n * (uint64_t)e->L.n_servers * 4, n, "rejection counts D2H");
 }
 int af_fetch_histograms(af_engine* e, uint32_t* out, uint64_t n) {
     if (e && e->ran && !e->L.collect_hist) return e->fail(AF_ERR_STATE, "histograms were not collected");

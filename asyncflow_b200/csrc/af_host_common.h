@@ -60,6 +60,7 @@ inline bool validate(const AfScenario& s, std::string& err) {
         AF_CHECK(v.out_edge >= 0 && v.out_edge < s.n_edges, "server %d: out_edge", i);
         AF_CHECK(v.n_endpoints >= 1 && v.endpoint_begin >= 0 && v.endpoint_begin + v.n_endpoints <= s.n_endpoints,
                  "server %d: endpoint range", i);
+        AF_CHECK(v.max_in_service >= 0, "server %d: max_in_service=%d must be >= 0 (0 = no admission limit)", i, v.max_in_service);
     }
     for (int i = 0; i < s.n_endpoints; ++i) {
         const AfEndpoint& p = s.endpoints[i];
@@ -107,6 +108,33 @@ inline bool validate_timeline(const AfScenario& s, const AfTimeline& t, std::str
         }
     }
 #undef AF_CHECK
+    return true;
+}
+
+// Does a launch shed requests at an admission limit somewhere (DESIGN.md §3.12)?  A scenario limit, or a sweep column
+// over AF_FIELD_SERVER_MAX_IN_SERVICE (even one of zeros): only such launches lay out the kernels' admission words.
+inline bool admission_launch(const AfScenario& s, const AfSweepColumn* cols, int32_t n_cols) {
+    for (int32_t i = 0; i < s.n_servers; ++i) if (s.servers[i].max_in_service > 0) return true;
+    for (int32_t c = 0; c < n_cols; ++c) if (cols[c].field == AF_FIELD_SERVER_MAX_IN_SERVICE) return true;
+    return false;
+}
+
+// af_sweep_upload's check of the AF_FIELD_SERVER_MAX_IN_SERVICE columns: every value an integer in [0, 2^31) (naming
+// the row).  Index ranges are checked with the other fields'.
+inline bool admission_sweep_fits(const AfSweepColumn* cols, int32_t n_cols, const double* vals, uint64_t n_rows, std::string& err) {
+    for (int32_t c = 0; c < n_cols; ++c) {
+        if (cols[c].field != AF_FIELD_SERVER_MAX_IN_SERVICE) continue;
+        for (uint64_t r = 0; r < n_rows; ++r) {
+            const double v = vals[r * (uint64_t)n_cols + (uint64_t)c];
+            if (!(v >= 0.0 && v <= 2147483647.0 && v == floor(v))) {      // (NaN fails the first test)
+                char b[200];
+                snprintf(b, sizeof b, "sweep: row %llu column %d (server_max_in_service, server %d): value %g is not an "
+                         "integer in [0, 2^31)", (unsigned long long)r, c, cols[c].index, v);
+                err = b;
+                return false;
+            }
+        }
+    }
     return true;
 }
 

@@ -110,7 +110,7 @@ constexpr int32_t NQ_TOTAL = 128;          // pending zero-delay items per repli
 // ---- read-only scenario tables (global memory, shared by all replicas; 16-byte multiples so that
 //      a record is one or a few 128-bit loads).  `c_*` = index into the lane's sweep-row copy, -1 = not swept.
 struct alignas(16) EdgeP { double mean, sigma, dropout; uint32_t meta; int16_t c_mean, c_sigma, c_drop, pad; uint32_t pad2[2]; };   // 48 B; meta: dist[0:3) | target_kind[3:5) | target_index[5:)
-struct alignas(16) ServerP { int32_t cpu_cores, ram_mb; uint32_t out_edge, ep_begin, n_ep; int32_t c_cores, c_ram, pad; };           // 32 B
+struct alignas(16) ServerP { int32_t cpu_cores, ram_mb; uint32_t out_edge, ep_begin, n_ep; int32_t c_cores, c_ram, max_in_service; }; // 32 B
 struct alignas(16) EndpointP { uint32_t step_begin, n_steps, total_ram; int32_t c_ram; };                                            // 16 B
 struct alignas(16) StepP { double dur; uint32_t kind; int32_t c_dur; };                                                              // 16 B
 struct alignas(16) SpikeP { double fire, delta; uint32_t edge; int32_t c_delta; uint32_t pad[2]; };                                  // 32 B
@@ -201,10 +201,17 @@ struct Cfg {
     // pool estimate, band group, timeline) are addressed by its id, replica_begin + W.local.
     const uint64_t* stream_of;
     uint64_t stream_first, stream_rows;
+    // admission limits (DESIGN.md §3.12), laid out only when adm != 0 (aflh::Tables.adm): per server, the 32-bit word
+    // o32_adm + s holds its limit minus the requests it admitted (ADM_FREE: no limit), the cold word c_rej + s the
+    // requests it shed, written to server_rejected[local * n_servers + s] at write-back
+    int32_t adm, o32_adm, c_rej;
+    uint32_t* server_rejected;
 };
 // Cfg.lb_algo of a launch that sweeps the load-balancer algorithm (AF_FIELD_LB_ALGORITHM; DESIGN.md §3.11): each replica
 // reads its own from the 32-bit word right after its LB order, o32_lb + n_lb_edges
 constexpr int32_t LB_PER_REPLICA = 2;
+// the admission word of a server without a limit (shed_at_door)
+constexpr int32_t ADM_FREE = INT32_MIN;
 
 
 #if defined(__CUDACC__)
@@ -433,6 +440,37 @@ AFL_IN void rq_release(St& W, const Mem& m, uint32_t s) {
 #else
 #define AFL_COLD static __attribute__((noinline))
 #endif
+// Admission limits (Cfg.adm; DESIGN.md §3.12; the full build only -- aflh::lean_launch).  A request leaves service when the handler hands it to the server's
+// out-edge, which only that server sends on, so the requests in service are the admitted ones minus the out-edge's send
+// count and the server's exits need no code of their own.  The server's 32-bit word holds its limit minus the requests
+// it admitted (ADM_FREE: no limit).
+// The dispatcher of server `sidx` takes a request: true when the server is at its limit (the request is shed at the door
+// and counted; the caller releases its record, as an edge dropout does), else the request is admitted.
+AFL_IN bool adm_shed(const Mem& m, uint32_t sidx, uint32_t out_edge) {
+    const int32_t w = AFL_C.o32_adm + (int32_t)sidx;
+    const int32_t budget = i32_ld(m, w);
+    if (budget == ADM_FREE) return false;
+    if ((int64_t)budget + (int64_t)ld_cg32(g32p(m, AFL_C.gi_sent + (int32_t)out_edge)) <= 0) {
+        c32_st(m, AFL_C.c_rej + (int32_t)sidx, c32_ld(m, AFL_C.c_rej + (int32_t)sidx) + 1u);
+        return true;
+    }
+    i32_st(m, w, budget - 1);
+    return false;
+}
+// start_replica: every server's word from the scenario (a sweep row overrides it after), no rejection yet
+AFL_COLD void adm_start(const Mem m) {
+    for (int32_t i = 0; i < AFL_C.n_servers; ++i) {
+        const int32_t lim = ro(AFL_C.servers + i).max_in_service;
+        i32_st(m, AFL_C.o32_adm + i, lim > 0 ? lim : ADM_FREE);
+        c32_st(m, AFL_C.c_rej + i, 0);
+    }
+}
+// write_back: the rejections of the replica in output slot `local`
+AFL_COLD void adm_write_back(const Mem m, uint64_t local) {
+    for (int32_t i = 0; i < AFL_C.n_servers; ++i)
+        AFL_C.server_rejected[local * (uint64_t)AFL_C.n_servers + (uint32_t)i] = c32_ld(m, AFL_C.c_rej + i);
+}
+
 AFL_COLD void fifo_push(const Mem m, int32_t w_head, int32_t w_tail, uint32_t s) {
     rq_next_set(m, s, NIL);
     const uint32_t tail = c32_ld(m, w_tail);
@@ -872,6 +910,7 @@ __device__ __forceinline__ void red_add(uint32_t* p, uint32_t v) { atomicAdd(p, 
 static inline void red_add(uint32_t* p, uint32_t v) { *p += v; }
 #endif
 
+
 // client: completion (client.py:62-69 + analyzer.py:83-125)
 template <bool kLatency, bool kLean>
 AFL_IN void complete(St& W, const Mem& m, uint32_t slot, double t0, uint32_t& lat_g) {
@@ -940,6 +979,7 @@ AFL_IN void start_replica(St& W, const Mem& m, uint64_t local_index) {
         c32_st(m, sq_word((uint32_t)i, SQ_CPUQ_HEAD), NIL); c32_st(m, sq_word((uint32_t)i, SQ_CPUQ_TAIL), NIL);
         c32_st(m, sq_word((uint32_t)i, SQ_RAMQ_NEED), 0);
     }
+    if (!kLean && C.adm) adm_start(m);
 #pragma unroll 1
     for (int32_t i = 0; i < C.n_servers + 2; ++i) {
         c32_st(m, ib_word((uint32_t)i, IB_HEAD), NIL); c32_st(m, ib_word((uint32_t)i, IB_TAIL), NIL); c32_st(m, ib_word((uint32_t)i, IB_PENDING), 1);
@@ -965,6 +1005,7 @@ AFL_IN void start_replica(St& W, const Mem& m, uint64_t local_index) {
         case AF_FIELD_SERVER_CPU_CORES: i32_st(m, sv_word((uint32_t)col.index, SV_CPU_FREE), (int32_t)v); break;
         case AF_FIELD_SERVER_RAM_MB: i32_st(m, sv_word((uint32_t)col.index, SV_RAM_FREE), (int32_t)v); break;
         case AF_FIELD_LB_COVERED: if (v == 0.0) { w32_st(m, C.o32_lb + col.index, NIL); uncovered = true; } break;
+        case AF_FIELD_SERVER_MAX_IN_SERVICE: if (!kLean) i32_st(m, C.o32_adm + col.index, v > 0.0 ? (int32_t)v : ADM_FREE); break;
         default: break;
         }
     }
@@ -1006,6 +1047,7 @@ AFL_IN void write_back(St& W, const Mem& m) {
         C.samp_sum[local * (uint64_t)C.n_series + (uint32_t)j] = sum;
         C.samp_max[local * (uint64_t)C.n_series + (uint32_t)j] = mx;
     }
+    if (!kLean && C.adm) adm_write_back(m, local);
     AfReplicaStats st;
     st.n_events = W.n_events; st.generated = W.generated; st.completed = W.completed;
     st.flags = W.flags; st.n_ticks = W.n_ticks; st.peak_events = W.peak_ev; st.peak_requests = W.peak_rq;
@@ -1262,33 +1304,37 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                 if (from_box) consumer_get(W, m, node);        // the dispatcher loops back to get() first (fused: the box is empty and
                                                                // the consumer already marked as waiting -- nothing to do)
                 const ServerP sp = ro(C.servers + sidx);
-                pack += 1;                                     // record_hop(SERVER)
-                uint32_t epi = 0;
-                if (!kLean && sp.n_ep > 1) {
-                    afr::Src src = afr::make_request(C.seed, W.replica, afr::P_SERVER, rid, pk_hops(pack));
-                    src.load(0);
-                    epi = (uint32_t)(((uint64_t)src.w.x * sp.n_ep) >> 32);
-                }
-                const uint32_t ep_global = sp.ep_begin + epi;
-                pack = (pack & 0xFFu) | (ep_global << 16);     // step 0, flags clear
-                const uint32_t total_ram = ep_total_ram(m, ep_global);
-                bool go = true;
-                if (total_ram) {                               // yield RAM.get(total_ram)
-                    if (!(can_fuse(W) && (int32_t)total_ram <= i32_ld(m, sv_word(sidx, SV_RAM_FREE)) && q_empty(W, m, sq_word(sidx, SQ_RAMQ_HEAD)))) {
-                        // cannot be served at once: join the queue, walk it
-                        rq_pack_set(W, m, slot, pack);
-                        if (q_empty(W, m, sq_word(sidx, SQ_RAMQ_HEAD))) c32_st(m, sq_word(sidx, SQ_RAMQ_NEED), total_ram);
-                        fifo_push(m, sq_word(sidx, SQ_RAMQ_HEAD), sq_word(sidx, SQ_RAMQ_TAIL), slot);
-                        W.n_waiting += 1;
-                        occ_add<kOcc>(W, m, occ_col(sidx, OC_RAM_WAIT), 1);
-                        ram_walk<kOcc>(W, m, sidx);
-                        go = false;
-                    } else {
-                        i32_st(m, sv_word(sidx, SV_RAM_FREE), i32_ld(m, sv_word(sidx, SV_RAM_FREE)) - (int32_t)total_ram);   // granted, and its get event would run next
-                        srv_gauge_add<kSampled, kDist, kOcc>(W, m, sidx, SV_RAM_IN_USE, (int32_t)total_ram);
+                const bool shed = !kLean && C.adm && adm_shed(m, sidx, sp.out_edge);
+                if (shed) rq_release(W, m, slot);             // shed at the door: the request is gone
+                else {
+                    pack += 1;                                     // record_hop(SERVER)
+                    uint32_t epi = 0;
+                    if (!kLean && sp.n_ep > 1) {
+                        afr::Src src = afr::make_request(C.seed, W.replica, afr::P_SERVER, rid, pk_hops(pack));
+                        src.load(0);
+                        epi = (uint32_t)(((uint64_t)src.w.x * sp.n_ep) >> 32);
                     }
+                    const uint32_t ep_global = sp.ep_begin + epi;
+                    pack = (pack & 0xFFu) | (ep_global << 16);     // step 0, flags clear
+                    const uint32_t total_ram = ep_total_ram(m, ep_global);
+                    bool go = true;
+                    if (total_ram) {                               // yield RAM.get(total_ram)
+                        if (!(can_fuse(W) && (int32_t)total_ram <= i32_ld(m, sv_word(sidx, SV_RAM_FREE)) && q_empty(W, m, sq_word(sidx, SQ_RAMQ_HEAD)))) {
+                            // cannot be served at once: join the queue, walk it
+                            rq_pack_set(W, m, slot, pack);
+                            if (q_empty(W, m, sq_word(sidx, SQ_RAMQ_HEAD))) c32_st(m, sq_word(sidx, SQ_RAMQ_NEED), total_ram);
+                            fifo_push(m, sq_word(sidx, SQ_RAMQ_HEAD), sq_word(sidx, SQ_RAMQ_TAIL), slot);
+                            W.n_waiting += 1;
+                            occ_add<kOcc>(W, m, occ_col(sidx, OC_RAM_WAIT), 1);
+                            ram_walk<kOcc>(W, m, sidx);
+                            go = false;
+                        } else {
+                            i32_st(m, sv_word(sidx, SV_RAM_FREE), i32_ld(m, sv_word(sidx, SV_RAM_FREE)) - (int32_t)total_ram);   // granted, and its get event would run next
+                            srv_gauge_add<kSampled, kDist, kOcc>(W, m, sidx, SV_RAM_IN_USE, (int32_t)total_ram);
+                        }
+                    }
+                    if (go) act = A_STEPS;
                 }
-                if (go) act = A_STEPS;
             } else {
                 pack += 1;                                     // record_hop(client / LB)
                 if (node == NODE_CLIENT) {

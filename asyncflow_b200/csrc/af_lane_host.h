@@ -15,6 +15,7 @@ struct Tables {
     std::vector<int32_t> lb; std::vector<afl::ColP> cols;
     int32_t n_row = 0;
     int32_t lb_algo_word = 0;      // 1: a column sweeps the LB algorithm (a 32-bit word per lane after the LB order)
+    int32_t adm = 0;               // 1: an admission limit somewhere (afh::admission_launch): a 32-bit word per server and lane
 };
 
 // Scenario (+ the sweep's columns) -> the kernel's read-only tables.  A column over a field the kernel
@@ -34,7 +35,8 @@ inline bool build_tables(const AfScenario& s, const AfSweepColumn* cols, int32_t
     for (int i = 0; i < s.n_servers; ++i) {
         const AfServer& a = s.servers[i]; afl::ServerP& v = t.servers[(size_t)i];
         v.cpu_cores = a.cpu_cores; v.ram_mb = a.ram_mb; v.out_edge = (uint32_t)a.out_edge;
-        v.ep_begin = (uint32_t)a.endpoint_begin; v.n_ep = (uint32_t)a.n_endpoints; v.c_cores = v.c_ram = -1; v.pad = 0;
+        v.ep_begin = (uint32_t)a.endpoint_begin; v.n_ep = (uint32_t)a.n_endpoints; v.c_cores = v.c_ram = -1; v.max_in_service = a.max_in_service;
+        if (a.max_in_service > 0) t.adm = 1;
     }
     t.endpoints.resize((size_t)s.n_endpoints);
     for (int i = 0; i < s.n_endpoints; ++i) {
@@ -76,6 +78,7 @@ inline bool build_tables(const AfScenario& s, const AfSweepColumn* cols, int32_t
                                    t.spikes[(size_t)i].c_delta = k.slot; break;
         case AF_FIELD_LB_COVERED: k.base = 1.0; break;
         case AF_FIELD_LB_ALGORITHM: k.base = s.lb_algo; t.lb_algo_word = 1; break;
+        case AF_FIELD_SERVER_MAX_IN_SERVICE: k.base = s.servers[i].max_in_service; t.adm = 1; break;
         default: err = "sweep: unknown field id"; return false;
         }
 #undef AFLH_SLOT
@@ -196,7 +199,7 @@ constexpr int32_t LANE_REQUEST_CAPACITY = 2048;
 inline int32_t fixed_lane_bytes(const AfScenario& s, const Tables& t) {
     const int32_t n_series = 3 * s.n_servers + s.n_edges;
     const int32_t fix64 = (s.n_spike_marks > 0 ? s.n_edges : 0) + t.n_row;
-    const int32_t fix32 = s.n_edges + afl::SV_WORDS * s.n_servers + s.n_lb_edges + t.lb_algo_word + (n_series + 31) / 32;
+    const int32_t fix32 = s.n_edges + afl::SV_WORDS * s.n_servers + s.n_lb_edges + t.lb_algo_word + t.adm * s.n_servers + (n_series + 31) / 32;
     return 8 * fix64 + 4 * fix32;
 }
 constexpr int32_t MIN_DYNAMIC_BYTES = 16 * 4 + 36 * 2;      // (a pool of 8 elements: 4 heap entries, 2 records and more)
@@ -210,9 +213,15 @@ inline void pool_split(const afl::Cfg& C, int32_t need, int32_t& ev_s, int32_t& 
 }
 
 // Does a launch qualify for the lean lane kernel (run_lane<*, *, true>)?  No spikes, no outages, no traced replica,
-// every edge normal or exponential, every server with one endpoint.  No sweep column can change any of these.
-inline bool lean_launch(const AfScenario& s, int32_t trace_replicas) {
+// every edge normal or exponential, every server with one endpoint, and no admission limit (a scenario limit or an
+// AF_FIELD_SERVER_MAX_IN_SERVICE column in `cols`: the lean loop leaves the check out, and the loop `bench.py` runs keeps
+// the instructions it had).  No other sweep column can change any of these.
+inline bool lean_launch(const AfScenario& s, int32_t trace_replicas, const AfSweepColumn* cols = nullptr, int32_t n_cols = 0) {
     if (s.n_spike_marks > 0 || s.n_outage_marks > 0 || trace_replicas > 0) return false;
+    for (int i = 0; i < s.n_servers; ++i)
+        if (s.servers[i].max_in_service > 0) return false;
+    for (int32_t c = 0; c < n_cols; ++c)
+        if (cols[c].field == AF_FIELD_SERVER_MAX_IN_SERVICE) return false;
     for (int i = 0; i < s.n_edges; ++i)
         if (s.edges[i].dist != AF_DIST_NORMAL && s.edges[i].dist != AF_DIST_EXPONENTIAL) return false;
     for (int i = 0; i < s.n_servers; ++i)
@@ -245,7 +254,7 @@ inline bool make_cfg(const AfScenario& s, const AfOptions& o, const Tables& t, i
     // fixed part of a lane's shared memory
     const int32_t fix64 = (C.n_spike > 0 ? C.n_edges : 0) + C.n_row;
     C.n_dirty = (C.n_series + 31) / 32;
-    const int32_t fix32 = C.n_edges + afl::SV_WORDS * C.n_servers + C.n_lb_edges + t.lb_algo_word + C.n_dirty;
+    const int32_t fix32 = C.n_edges + afl::SV_WORDS * C.n_servers + C.n_lb_edges + t.lb_algo_word + t.adm * C.n_servers + C.n_dirty;
     int32_t nq_s = 0;                                // zero-delay items: ties only -- the ring starts in the global tier
     const int32_t rest = lane_bytes - 8 * fix64 - 4 * fix32;
     // the rest is the pool: 16-byte elements shared by the heap and the request records, split per replica
@@ -276,6 +285,7 @@ inline bool make_cfg(const AfScenario& s, const AfOptions& o, const Tables& t, i
     C.o32_srv = w; w += afl::SV_WORDS * C.n_servers;
     C.o32_lb = w; w += C.n_lb_edges + t.lb_algo_word;
     C.o32_dirty = w; w += C.n_dirty;
+    C.adm = t.adm; C.o32_adm = w; w += t.adm * C.n_servers;
     C.n32 = w;
     C.warp_bytes = (C.n128 * 16 + C.n64 * 8 + C.n32 * 4) * lanes;
     // global tier: 128-bit region (events, request records), 64-bit region (now-queue), 32-bit region (links, cold words).
@@ -289,7 +299,8 @@ inline bool make_cfg(const AfScenario& s, const AfOptions& o, const Tables& t, i
     int32_t hcount = rq_total;                       // the `next` link of every record slot
     C.g32_cold = hcount;
     C.c_srvq = 0; C.c_inbox = C.c_srvq + afl::SQ_WORDS * C.n_servers; C.c_drop = C.c_inbox + afl::IB_WORDS * (C.n_servers + 2);
-    hcount += C.c_drop + C.n_edges;
+    C.c_rej = C.c_drop + C.n_edges;
+    hcount += C.c_rej + t.adm * C.n_servers;
     C.gi_smax = hcount; hcount += C.n_series;
     C.gi_sent = hcount; hcount += C.n_edges;
     C.gn32 = hcount;

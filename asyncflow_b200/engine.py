@@ -154,6 +154,12 @@ class Engine:
                     "af_fetch_edge_counts")
         return sent, dropped
 
+    def server_rejected(self, out: np.ndarray | None = None) -> np.ndarray:
+        """Requests each server shed at its admission limit, ``[n, n_servers]`` -- ``af_fetch_server_rejected``."""
+        out = np.empty((self._n, self.flat.n_servers), dtype=np.uint32) if out is None else out
+        self._check(self._lib.af_fetch_server_rejected(self._h, out.ctypes.data, self._n), "af_fetch_server_rejected")
+        return out
+
     def histograms(self) -> np.ndarray:
         out = np.empty((self._n, K.AF_HIST_BINS), dtype=np.uint32)
         self._check(self._lib.af_fetch_histograms(self._h, out.ctypes.data, self._n), "af_fetch_histograms")

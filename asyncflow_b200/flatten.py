@@ -74,6 +74,32 @@ def _lb_position(flat: "FlatScenario", server_id: str) -> int:
     raise KeyError(msg)
 
 
+def _limit(x: Any) -> float:
+    """An admission limit as a float, NaN unless it is an integer in [0, 2**31) (bools refused)."""
+    if isinstance(x, (bool, np.bool_)):
+        return np.nan
+    try:
+        v = float(x)
+    except (TypeError, ValueError):
+        return np.nan
+    return v if v == v and 0.0 <= v < 2.0 ** 31 and v == int(v) else np.nan
+
+
+def set_admission(flat: "FlatScenario", admission: dict[str, int] | None) -> None:
+    """The scenario's admission limits (DESIGN.md §3.12): ``admission[server_id]`` requests in service at once, 0 = no
+    limit; servers left out keep theirs.  ``KeyError`` for an unknown server, ``ValueError`` for a limit that is not an
+    integer in [0, 2**31)."""
+    for sid, v in (admission or {}).items():
+        if sid not in flat.server_ids:
+            msg = f"admission: no server {sid!r} (servers: {list(flat.server_ids)})"
+            raise KeyError(msg)
+        lim = _limit(v)
+        if lim != lim:
+            msg = f"admission: server {sid!r}: limit {v!r} is not an integer in [0, 2**31)"
+            raise ValueError(msg)
+        flat.pod.servers[flat.server_ids.index(sid)].max_in_service = int(lim)
+
+
 def _rv(d: dict) -> tuple[str, float, float]:
     dist = _s(d.get("distribution") or "poisson")
     var = d.get("variance")
@@ -414,7 +440,8 @@ class SweepSpec:
     ``("endpoint_ram", server_id, endpoint_idx)``, ``("spike_delta", event_id)``,
     ``("event_start"|"event_end", event_id)`` (the ``t_start`` / ``t_end`` of a spike or an outage),
     ``("lb_covered", server_id)`` (1: behind the load balancer as in the scenario, 0: not; bools accepted) and
-    ``("lb_algorithm",)`` (``"round_robin"`` or ``"least_connection"``, enum members or ``K.LB_*`` codes accepted).
+    ``("lb_algorithm",)`` (``"round_robin"`` or ``"least_connection"``, enum members or ``K.LB_*`` codes accepted) and
+    ``("server_max_in_service", server_id)`` (the server's admission limit, an integer >= 0, 0 = none; DESIGN.md §3.12).
 
     A row that uncovers a server simulates the scenario without the load balancer's edge to it (:meth:`payload_for`):
     its round-robin order is the scenario's with that edge left out, and an outage of that server is a no-op.  The
@@ -438,6 +465,7 @@ class SweepSpec:
         vals: list[np.ndarray] = []
         keys = [tuple(sel) if not isinstance(sel, str) else (sel,) for sel in columns]
         arrays = [self._lb_values(flat, sel, v) if sel[0] in ("lb_covered", "lb_algorithm")
+                  else self._limits(flat, sel, v) if sel[0] in K.ADMISSION_FIELDS
                   else np.ascontiguousarray(np.broadcast_to(np.asarray(v, dtype=np.float64), (self.n_replicas,)))
                   for sel, v in zip(keys, columns.values())]
         self.covered = self._covered(flat, keys, arrays)
@@ -478,7 +506,7 @@ class SweepSpec:
                 raise KeyError(msg)
             self.selectors.append((sel, arr))
             for t in targets:
-                cols.append(((K.LB_FIELDS if name in K.LB_FIELDS else K.FIELDS)[name], t))
+                cols.append(({**K.FIELDS, **K.LB_FIELDS, **K.ADMISSION_FIELDS}[name], t))
                 vals.append(arr)
         self.n_columns = len(cols)
         self.values = (np.ascontiguousarray(np.stack(vals, axis=1)) if vals
@@ -521,6 +549,30 @@ class SweepSpec:
             msg = f"sweep row {r}: {sel!r} = {raw[r]!r}: a server is covered (1) or not (0)"
             raise ValueError(msg)
         return np.ascontiguousarray(out)
+
+    def _limits(self, flat: FlatScenario, sel: tuple, v: Any) -> np.ndarray:
+        """An admission-limit column: integers in [0, 2**31) as floats (``KeyError`` / ``ValueError`` naming the row)."""
+        if len(sel) != 2 or sel[1] not in flat.server_ids:
+            msg = f"sweep column {sel!r}: no server {sel[1] if len(sel) > 1 else None!r} (servers: {list(flat.server_ids)})"
+            raise KeyError(msg)
+        raw = np.broadcast_to(np.asarray(v, dtype=object), (self.n_replicas,))
+        out = np.array([_limit(x) for x in raw], dtype=np.float64)
+        bad = np.isnan(out)
+        if bad.any():
+            r = int(np.flatnonzero(bad)[0])
+            msg = f"sweep row {r}: {sel!r} = {raw[r]!r}: an admission limit is an integer in [0, 2**31) (0: none)"
+            raise ValueError(msg)
+        return out
+
+    def admission_for(self, replica: int) -> dict[str, int]:
+        """Row ``replica``'s admission limits ``{server_id: limit}`` from this spec's columns (zeros included)."""
+        return {sel[1]: int(arr[replica]) for sel, arr in self.selectors if sel[0] in K.ADMISSION_FIELDS}
+
+    def payload_and_admission(self, payload: Any, replica: int) -> tuple[dict, dict[str, int]]:
+        """Row ``replica`` as the oracle takes it: the row's payload (:meth:`payload_for` without the admission
+        columns) and its admission limits, ``{server_id: limit}`` (0: none).  The reference cannot express a limit, so a
+        capped row has no payload of its own."""
+        return self._payload(payload, replica), self.admission_for(replica)
 
     def _covered(self, flat: FlatScenario, keys: list[tuple], arrays: list[np.ndarray]) -> np.ndarray | None:
         """[R, len(flat.lb_edges)] bool: the LB edges each row keeps (``None`` without ``lb_covered`` columns), checked
@@ -632,7 +684,17 @@ class SweepSpec:
         ``GpuSimulationRunner``) simulates exactly what row ``replica`` of the sweep simulates;
         it is how a sweep point is handed back to the reference for inspection, and how the parity
         tests build the oracle's input.  ``payload`` is the base scenario the sweep was made from.
+        A row with an admission limit has no such payload (the reference has no limits): ``ValueError``; use
+        :meth:`payload_and_admission`.
         """
+        capped = {sid: v for sid, v in self.admission_for(replica).items() if v}
+        if capped:
+            msg = (f"sweep row {replica} sets admission limits {capped}, which a payload cannot express; "
+                   "payload_and_admission() returns the payload and the limits")
+            raise ValueError(msg)
+        return self._payload(payload, replica)
+
+    def _payload(self, payload: Any, replica: int) -> dict:
         import copy  # noqa: PLC0415
 
         p = copy.deepcopy(_as_dict(payload))

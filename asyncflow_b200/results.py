@@ -20,7 +20,7 @@ proved by ``tests/unit/metrics/test_analyzer.py:34-126``).
 from __future__ import annotations
 
 from collections import defaultdict
-from dataclasses import dataclass
+from dataclasses import dataclass, field
 from types import SimpleNamespace
 from typing import Any
 
@@ -170,6 +170,7 @@ class ReplicaResults:
     edge_dropped: dict[str, int]
     n_events: int
     flags: int
+    server_rejected: dict[str, int] = field(default_factory=dict)   # requests each server shed at its admission limit
 
     # -- analyzer-compatible getters (metrics/analyzer.py:147-262) -------------
     def list_server_ids(self) -> list[str]:
@@ -297,6 +298,8 @@ class SweepResults:
         self.throughput = throughput
         self.histograms = histograms
         self.replica_begin = replica_begin
+        # requests each server shed at its admission limit, [n, n_servers] u32 (zeros without limits; DESIGN.md §3.12)
+        self.server_rejected = np.zeros((len(stats), flat.n_servers if flat is not None else 0), dtype=np.uint32)
         self.rows: np.ndarray | None = None      # sweep row of each result row (set by SweepRunner)
         self.streams: np.ndarray | None = None   # random stream of each result row (SweepRunner.stream_ids; set by collect)
         self.traced: list[ReplicaResults] = []    # full clocks + sampled series of the first `trace_replicas` replica ids
@@ -465,6 +468,7 @@ class SweepResults:
                            self.samp_sum[index], self.samp_max[index], g(self.throughput), g(self.histograms),
                            self.replica_begin)
         out.traced = self.traced
+        out.server_rejected = self.server_rejected[index]
         out.streams = g(self.streams)
         out.band_count, out.band_sum, out.band_sumsq = self.band_count, self.band_sum, self.band_sumsq
         out.lat_window_s, out.lat_hist, out.lat_sum_hi, out.lat_sum_lo = (self.lat_window_s, self.lat_hist,
@@ -664,6 +668,7 @@ class SweepResults:
             np.concatenate([p.edge_dropped for p in parts]), np.concatenate([p.samp_sum for p in parts]),
             np.concatenate([p.samp_max for p in parts]), cat([p.throughput for p in parts]),
             cat([p.histograms for p in parts]), f.replica_begin)
+        out.server_rejected = np.concatenate([p.server_rejected for p in parts])
         if all(p.streams is not None for p in parts):
             out.streams = np.concatenate([p.streams for p in parts])
         if all(p.band_count is not None for p in parts):      # integer sums over disjoint replicas: they add exactly

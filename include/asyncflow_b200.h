@@ -38,7 +38,7 @@
 extern "C" {
 #endif
 
-#define AF_ABI_VERSION 9
+#define AF_ABI_VERSION 10
 
 typedef enum AfStatus {
     AF_OK = 0,
@@ -80,7 +80,8 @@ typedef struct AfServer {        /* schemas/topology/nodes.py:52-104 */
     int32_t out_edge;            /* the server's single outgoing edge              */
     int32_t endpoint_begin;      /* first AfEndpoint of this server                */
     int32_t n_endpoints;
-    int32_t reserved;
+    int32_t max_in_service;      /* admission limit: requests in service at once   *
+                                  * (0 = no limit; see AF_FIELD_SERVER_MAX_IN_SERVICE) */
 } AfServer;
 
 typedef struct AfEndpoint {      /* schemas/topology/endpoint.py:92-102 */
@@ -150,7 +151,8 @@ enum {
     AF_FIELD_SPIKE_DELTA = 10,   /* index = spike mark; sign is kept by the engine */
     AF_FIELD_LB_COVERED = 11,    /* index = position in lb_edges; 1 = behind the LB as in the scenario, 0 = not */
     AF_FIELD_LB_ALGORITHM = 12,  /* index 0; an AF_LB_* algorithm (round robin or least connections)           */
-    AF_FIELD_COUNT = 13
+    AF_FIELD_SERVER_MAX_IN_SERVICE = 13,  /* index = server; an admission limit, 0 = none (AfServer.max_in_service) */
+    AF_FIELD_COUNT = 14
 };
 /* Load-balancer rows (DESIGN.md §3.11).  A replica whose row sets AF_FIELD_LB_COVERED of position k to 0 runs without
  * the LB edge lb_edges[k]: its round-robin order is lb_edges with the uncovered edges left out; the server and its other
@@ -159,6 +161,14 @@ enum {
  * out of range, a value other than 0 or 1, and a row that covers no edge (naming the row).  af_run refuses a launch in
  * which a row uncovers an LB edge that the outage marks it runs with (its timeline row, else the scenario's) still name:
  * give such rows timeline rows whose marks for that server have lb_edge = -1. */
+/* Admission limits (DESIGN.md §3.12).  A server with a limit L > 0 (AfServer.max_in_service, or the replica's
+ * AF_FIELD_SERVER_MAX_IN_SERVICE value) admits a request its dispatcher takes from the inbox only while fewer than L
+ * requests are in service there -- from admission until the handler hands them to the server's out-edge, RAM and core
+ * waits included.  A request beyond the limit is shed at the door: no hop, no endpoint draw, no handler; it never
+ * reaches the client (as an edge dropout), its in-edge still counts it as sent, and af_fetch_server_rejected counts it.
+ * No random number is drawn, so replicas sharing a stream see the same traffic whatever their limits.  Replicas without
+ * a row keep the scenario's limits.  af_scenario_upload refuses a negative max_in_service; af_sweep_upload refuses an
+ * index out of range and a value that is not an integer in [0, 2^31) (naming the row). */
 typedef struct AfSweepColumn { int32_t field; int32_t index; } AfSweepColumn;
 typedef struct AfSweep {
     int32_t n_columns;
@@ -283,6 +293,8 @@ int af_last_run_passes(af_engine* e, AfRunPasses* out);
 int af_fetch_stats(af_engine* e, AfReplicaStats* out, uint64_t n);
 int af_fetch_edge_counts(af_engine* e, uint32_t* sent, uint32_t* dropped, uint64_t n); /* [n][n_edges] */
 int af_fetch_histograms(af_engine* e, uint32_t* out, uint64_t n);   /* [n][AF_HIST_BINS] */
+/* requests each server shed at its admission limit: [n][n_servers] (all 0 when the run had no limit) */
+int af_fetch_server_rejected(af_engine* e, uint32_t* out, uint64_t n);
 int af_fetch_throughput(af_engine* e, uint32_t* out, uint64_t n);   /* [n][horizon_s]    */
 /* sampled-metric aggregates over ticks: per replica, per series j:
  *   j <  3*n_servers : server j/3, metric j%3 in {ready_queue_len, event_loop_io_sleep, ram_in_use}
