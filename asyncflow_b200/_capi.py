@@ -11,7 +11,7 @@ from __future__ import annotations
 import ctypes as C
 from pathlib import Path
 
-AF_ABI_VERSION = 10
+AF_ABI_VERSION = 11
 AF_HIST_BINS = 4096
 AF_HIST_SUB_BITS = 7
 AF_HIST_MIN_EXP = -20
@@ -35,6 +35,9 @@ LB_FIELDS = {"lb_covered": 11, "lb_algorithm": 12}
 #: from FIELDS: the reference has no such parameter, so a row that sets one runs a scenario it cannot express
 #: (DESIGN.md §3.12).
 ADMISSION_FIELDS = {"server_max_in_service": 13}
+#: request deadlines (AF_FIELD_SERVER_DEADLINE, per server) and the client timeout (AF_FIELD_CLIENT_TIMEOUT), in seconds,
+#: 0 = none.  Kept apart from FIELDS for the same reason (DESIGN.md §3.13).
+DEADLINE_FIELDS = {"server_deadline": 14, "client_timeout": 15}
 FLAG_EVENT_OVERFLOW, FLAG_REQUEST_OVERFLOW, FLAG_TRACE_TRUNCATED, FLAG_NOWQ_OVERFLOW, FLAG_LB_EMPTY = 1, 2, 4, 8, 16
 MODE_AUTO, MODE_WARP, MODE_LANE, MODE_TWO_PASS = 0, 1, 2, 3
 SELFTEST_EDGE, SELFTEST_GEN_UNIFORM, SELFTEST_GEN_USERS, SELFTEST_ENDPOINT = 0, 1, 2, 3
@@ -50,7 +53,8 @@ class AfEdge(C.Structure):
 
 class AfServer(C.Structure):
     _fields_ = [("cpu_cores", C.c_int32), ("ram_mb", C.c_int32), ("out_edge", C.c_int32),
-                ("endpoint_begin", C.c_int32), ("n_endpoints", C.c_int32), ("max_in_service", C.c_int32)]
+                ("endpoint_begin", C.c_int32), ("n_endpoints", C.c_int32), ("max_in_service", C.c_int32),
+                ("deadline", C.c_double)]
 
 
 class AfEndpoint(C.Structure):
@@ -83,7 +87,7 @@ class AfScenario(C.Structure):
         ("edges", C.POINTER(AfEdge)), ("servers", C.POINTER(AfServer)),
         ("endpoints", C.POINTER(AfEndpoint)), ("steps", C.POINTER(AfStep)),
         ("lb_edges", C.POINTER(C.c_int32)), ("spike_marks", C.POINTER(AfSpikeMark)),
-        ("outage_marks", C.POINTER(AfOutageMark)),
+        ("outage_marks", C.POINTER(AfOutageMark)), ("client_timeout", C.c_double),
     ]
 
 
@@ -155,7 +159,7 @@ EXPORTS = [
     "af_fetch_trace_series", "af_reduce_histograms", "af_engine_set_mode", "af_last_run_passes",
     "af_selftest_rng", "af_bands_upload", "af_fetch_bands", "af_bands_configure", "af_fetch_latency_bands",
     "af_dist_bands_configure", "af_fetch_dist_bands", "af_occupancy_configure", "af_fetch_occupancy",
-    "af_timeline_upload", "af_streams_upload", "af_fetch_server_rejected",
+    "af_timeline_upload", "af_streams_upload", "af_fetch_server_rejected", "af_fetch_server_expired", "af_fetch_late",
 ]
 
 _lib = None
@@ -194,6 +198,8 @@ def load() -> C.CDLL:
     lib.af_fetch_edge_counts.argtypes = [vp, vp, vp, u64]
     lib.af_fetch_histograms.argtypes = [vp, vp, u64]
     lib.af_fetch_server_rejected.argtypes = [vp, vp, u64]
+    lib.af_fetch_server_expired.argtypes = [vp, vp, u64]
+    lib.af_fetch_late.argtypes = [vp, vp, u64]
     lib.af_fetch_throughput.argtypes = [vp, vp, u64]
     lib.af_fetch_sampled.argtypes = [vp, vp, vp, u64]
     lib.af_fetch_trace_clocks.argtypes = [vp, u64, vp, u64, C.POINTER(u64)]

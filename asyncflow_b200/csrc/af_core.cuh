@@ -114,8 +114,10 @@ AF_IN uint32_t mk_payload(uint32_t kind, uint32_t aux, uint32_t slot) {
     return (kind << 29) | (aux << SLOT_BITS) | slot;
 }
 
-// ---- request record pack: hops[0:8) step[8:16) ep[16:28) core[28] io[29] ----
+// ---- request record pack: hops[0:8) step[8:16) ep[16:28) core[28] io[29] wait[30] expired[31] ----
 constexpr uint32_t PK_CORE = 1u << 28, PK_IO = 1u << 29;
+constexpr uint32_t PK_EXPIRED = 1u << 31;   // past its server's deadline: the handler's tail runs, no forward (§3.13)
+constexpr double INF_DEADLINE = __builtin_huge_val();   // ServerS.deadline / State.timeout of "none"
 AF_IN uint32_t pk_hops(uint32_t p) { return p & 0xFFu; }
 AF_IN uint32_t pk_step(uint32_t p) { return (p >> 8) & 0xFFu; }
 AF_IN uint32_t pk_ep(uint32_t p) { return (p >> 16) & 0xFFFu; }
@@ -137,7 +139,8 @@ struct ServerS {          // 64 B
     // admission limit (DESIGN.md §3.12): admissions left before the server sheds (0xFFFFFFFF: no limit; one per request
     // in service), requests shed
     uint32_t adm_left, rejected;
-    uint32_t pad;
+    // requests dropped past the server's deadline (DESIGN.md §3.13; the deadline itself: tbl_deadline)
+    uint32_t expired;
 };
 struct EndpointS { uint32_t step_begin, n_steps, total_ram, pad; }; // 16 B
 struct StepS { double dur; uint32_t kind, pad; };                   // 16 B
@@ -191,6 +194,9 @@ struct State {
     uint32_t dist_bins, dist_pad;
     // occupancy integrals: the replica's output row (nullptr: off; afl::occ_add, DESIGN.md §3.8), 2^f
     uint64_t* occ; double occ_scale;
+    // client timeout (DESIGN.md §3.13; +inf: none) and the completions later than it
+    double timeout;
+    uint32_t late, late_pad;
 };
 
 // Everything the kernel needs to know about sizes; built on the host.
@@ -234,6 +240,10 @@ struct BandArgs {
     // requests each server shed at its admission limit (nullptr: the launch has no limit; DESIGN.md §3.12):
     // [n_replicas][n_servers] u32, written with the replica's other outputs
     uint32_t* server_rejected;
+    // requests each server dropped past its deadline, [n_replicas][n_servers] u32, and completions later than the client
+    // timeout, [n_replicas] u32 (nullptr: the launch has neither; DESIGN.md §3.13)
+    uint32_t* server_expired; uint32_t* late;
+    double client_timeout;         // the scenario's (0: none)
 };
 
 // Per-replica timelines of a launch (af_sim_kernel's parameter; rows == 0: none): replica first + r, r < rows, copies its
@@ -271,7 +281,8 @@ inline void layout_finalize(Layout& L) {
     L.off_rq_next = o;  o += 4 * L.rq_smem;
     L.off_samp_max = o; o += 4 * L.n_series;
     L.off_lb = o;       o += 4 * L.n_lb_edges;
-    L.warp_bytes = align_up(o, 16);
+    o = align_up(o, 8) + 8 * L.n_servers;  // each server's deadline (tbl_deadline: no Layout field, so that no
+    L.warp_bytes = align_up(o, 16);         // __constant__ offset of the lane kernel's moves)
 }
 
 // Device-global pointers (read-only scenario, sweep rows, spill tiers, outputs).
@@ -327,6 +338,10 @@ AF_TBL(tbl_spike, SpikeS, off_spike)
 AF_TBL(tbl_outage, OutageS, off_outage)
 AF_TBL(tbl_samp_sum, uint64_t, off_samp_sum)
 AF_TBL(tbl_samp_max, uint32_t, off_samp_max)
+// each server's deadline in seconds (+inf: none; DESIGN.md §3.13), f64, right after the LB order
+AF_IN double* tbl_deadline(State& W) {
+    return reinterpret_cast<double*>(reinterpret_cast<unsigned char*>(&W) + align_up(AF_L.off_lb + 4 * AF_L.n_lb_edges, 8));
+}
 AF_TBL(tbl_nq, uint64_t, off_nq)
 AF_TBL(tbl_inbox, InboxS, off_inbox)
 AF_IN uint32_t* tbl_band_prev(State& W) { return reinterpret_cast<uint32_t*>(reinterpret_cast<unsigned char*>(&W) + W.band_prev_off); }
@@ -706,6 +721,14 @@ AF_FN void run_steps(State& W, uint32_t slot, uint32_t sidx, uint32_t rid, uint3
                         return;
                     }
                 }
+                // the request holds a core: past its server's deadline it abandons -- the tail of the handler as it
+                // stands (core, then RAM), no forward (DESIGN.md §3.13)
+                // (the start time is read from the record only for a server with a deadline: a register across every
+                //  call of run_steps costs af_sim_kernel a spill)
+                if (AF_UNLIKELY(tbl_deadline(W)[sidx] < INF_DEADLINE) && W.now - rq_load(W, slot).t0 > tbl_deadline(W)[sidx]) {
+                    pack = (pack & ~0xFF00u) | (ep.n_steps << 8) | PK_EXPIRED;
+                    continue;
+                }
                 rq_set_pack(W, slot, pack);
                 push(W, W.now + sp.dur, mk_payload(K_STEP_END, sidx, slot));
                 return;
@@ -741,7 +764,8 @@ AF_FN void run_steps(State& W, uint32_t slot, uint32_t sidx, uint32_t rid, uint3
             if (!can_fuse(W)) { nq_push(W, I_RAM_PUT, sidx, slot); return; }
             if (AF_UNLIKELY(S.ramq_head != NIL)) ram_walk(W, S, sidx);   // the put event would run next: waiters, then forward
         }
-        S.adm_left += 1;                             // out of service: handed to the out-edge
+        S.adm_left += 1;                             // out of service: handed to the out-edge, or dropped past its deadline
+        if (AF_UNLIKELY(pack & PK_EXPIRED)) { S.expired += 1; rq_release(W, slot); return; }
         edge_send(W, slot, S.out_edge, rid, pk_hops(pack));
         return;
     }
@@ -814,6 +838,7 @@ AF_IN void complete(State& W, uint32_t slot, double t0) {
     W.lat_sumsq += lat * lat;
     if (lat < W.lat_min) W.lat_min = lat;
     if (lat > W.lat_max) W.lat_max = lat;
+    if (lat > W.timeout) W.late += 1;                // later than the client timeout (DESIGN.md §3.13)
     const bool traced = W.traced != 0;
     if (traced && (int32_t)(done - 1) >= AF_L.trace_clock_cap) W.flags |= AF_FLAG_TRACE_TRUNCATED;
     if (lane_id() == 0) {
@@ -913,6 +938,7 @@ AF_IN void run_item(State& W, uint32_t item) {
         ram_walk(W, S, aux);
         ReqRec r = rq_load(W, slot);
         S.adm_left += 1;
+        if (AF_UNLIKELY(r.pack & PK_EXPIRED)) { S.expired += 1; rq_release(W, slot); return; }   // past its deadline: no forward
         edge_send(W, slot, S.out_edge, r.rid, pk_hops(r.pack));
     }
 }
@@ -1116,7 +1142,7 @@ AF_IN void bind(State& W, unsigned char* ws, uint64_t warp_slot) {
 }
 
 // `spikes` / `outages`: the replica's mark tables (its timeline row, or the scenario's)
-AF_FN void load_params(State& W, const AfSpikeMark* spikes, const AfOutageMark* outages) {
+AF_FN void load_params(State& W, const AfSpikeMark* spikes, const AfOutageMark* outages, double client_timeout) {
     AF_SHARED(&W);
     const int lane = lane_id();
 #pragma unroll 1
@@ -1135,7 +1161,9 @@ AF_FN void load_params(State& W, const AfSpikeMark* spikes, const AfOutageMark* 
         s.cpu_free = a.cpu_cores; s.ram_free = a.ram_mb; s.ready_q = 0; s.io_q = 0; s.ram_in_use = 0;
         s.ramq_head = s.ramq_tail = s.cpuq_head = s.cpuq_tail = NIL;
         s.out_edge = (uint32_t)a.out_edge; s.ep_begin = (uint32_t)a.endpoint_begin; s.n_ep = (uint32_t)a.n_endpoints;
-        s.ramq_head_need = 0; s.adm_left = a.max_in_service > 0 ? (uint32_t)a.max_in_service : 0xFFFFFFFFu; s.rejected = 0; s.pad = 0;
+        s.ramq_head_need = 0; s.adm_left = a.max_in_service > 0 ? (uint32_t)a.max_in_service : 0xFFFFFFFFu; s.rejected = 0;
+        s.expired = 0;
+        tbl_deadline(W)[i] = a.deadline > 0.0 ? a.deadline : INF_DEADLINE;
         tbl_server(W)[i] = s;
     }
 #pragma unroll 1
@@ -1173,6 +1201,7 @@ AF_FN void load_params(State& W, const AfSpikeMark* spikes, const AfOutageMark* 
     w_sync();
     W.users_mean = AF_L.users_mean; W.users_sigma = AF_L.users_sigma; W.rate_per_user = AF_L.rate_per_user;
     W.lb_algo = AF_L.lb_algo;
+    W.timeout = client_timeout > 0.0 ? client_timeout : INF_DEADLINE; W.late = 0; W.late_pad = 0;
     // sweep overrides of this replica (uniform: every lane applies every column)
     const uint64_t replica = AF_G.replica_begin + W.local;     // (W.replica is its stream)
     if (AF_L.n_sweep_cols > 0 && replica >= AF_G.sweep_first && replica - AF_G.sweep_first < AF_G.sweep_rows) {
@@ -1198,6 +1227,8 @@ AF_FN void load_params(State& W, const AfSpikeMark* spikes, const AfOutageMark* 
             case AF_FIELD_LB_COVERED: if (v == 0.0) { tbl_lb(W)[col.index] = NIL; uncovered = true; } break;
             case AF_FIELD_LB_ALGORITHM: W.lb_algo = (int32_t)v; break;
             case AF_FIELD_SERVER_MAX_IN_SERVICE: tbl_server(W)[col.index].adm_left = v > 0.0 ? (uint32_t)v : 0xFFFFFFFFu; break;
+            case AF_FIELD_SERVER_DEADLINE: tbl_deadline(W)[col.index] = v > 0.0 ? v : INF_DEADLINE; break;
+            case AF_FIELD_CLIENT_TIMEOUT: W.timeout = v > 0.0 ? v : INF_DEADLINE; break;
             default: break;
             }
         }
@@ -1290,7 +1321,8 @@ AF_IN void run_replica(State& W, uint64_t local_index, const BandArgs& band, con
     {
         const uint64_t r = id - tl.first;
         const bool own = r < tl.rows;
-        load_params(W, own ? tl.spikes + r * (uint64_t)AF_L.n_spike : AF_G.spikes, own ? tl.outages + r * (uint64_t)AF_L.n_outage : AF_G.outages);
+        load_params(W, own ? tl.spikes + r * (uint64_t)AF_L.n_spike : AF_G.spikes, own ? tl.outages + r * (uint64_t)AF_L.n_outage : AF_G.outages,
+                    band.client_timeout);
     }
 
     // start order of the reference (simulation_runner.py:339-342, 301-336):
@@ -1361,6 +1393,12 @@ AF_IN void run_replica(State& W, uint64_t local_index, const BandArgs& band, con
     if (band.server_rejected != nullptr) {
         for (int32_t i = lane_id(); i < AF_L.n_servers; i += WARP)
             band.server_rejected[local_index * (uint64_t)AF_L.n_servers + (uint32_t)i] = tbl_server(W)[i].rejected;
+        w_sync();
+    }
+    if (band.server_expired != nullptr) {
+        for (int32_t i = lane_id(); i < AF_L.n_servers; i += WARP)
+            band.server_expired[local_index * (uint64_t)AF_L.n_servers + (uint32_t)i] = tbl_server(W)[i].expired;
+        if (lane_id() == 0) band.late[local_index] = W.late;
         w_sync();
     }
 }

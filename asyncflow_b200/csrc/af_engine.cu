@@ -431,6 +431,10 @@ struct af_engine {
     // requests shed at admission limits, [n][n_servers] (DESIGN.md §3.12); written by launches with a limit somewhere
     DevBuf d_rejected;
     bool last_adm = false;
+    // requests dropped past server deadlines [n][n_servers], completions later than the client timeout [n] (DESIGN.md
+    // §3.13); written by launches with a deadline or a timeout somewhere, which also upload the lane's dl_base table
+    DevBuf d_expired, d_late, d_l_dl;
+    bool last_dl = false;
     bool last_occ = false; int32_t last_occ_bits = 0, last_occ_cols = 0;
 
     int fail(int code, const std::string& m) { err = m; return code; }
@@ -515,7 +519,8 @@ void af_engine_destroy(af_engine* e) {
                       &e->d_tclk, &e->d_tser, &e->d_tcnt, &e->d_counter, &e->d_htot,
                       &e->d_okey, &e->d_oidx, &e->d_order, &e->d_okey64, &e->d_sort_tmp,
                       &e->d_band_group, &e->d_band, &e->d_band_from, &e->d_lat, &e->d_lat_from,
-                      &e->d_dist_slot, &e->d_dist, &e->d_occ, &e->d_tl_spikes, &e->d_tl_l_spikes, &e->d_tl_outages, &e->d_streams};
+                      &e->d_dist_slot, &e->d_dist, &e->d_occ, &e->d_tl_spikes, &e->d_tl_l_spikes, &e->d_tl_outages, &e->d_streams,
+                      &e->d_expired, &e->d_late, &e->d_l_dl};
     for (DevBuf* b : bufs) b->release();
     cudaEventDestroy(e->ev_begin); cudaEventDestroy(e->ev_sim); cudaEventDestroy(e->ev_end);
     cudaStreamDestroy(e->stream);
@@ -589,6 +594,8 @@ int af_sweep_upload(af_engine* e, const AfSweep* sw, uint64_t first_replica) {
         case AF_FIELD_SPIKE_DELTA: lim = s.n_spike_marks; break;
         case AF_FIELD_LB_COVERED: lim = s.n_lb_edges; break;
         case AF_FIELD_LB_ALGORITHM: lim = 1; break;
+        case AF_FIELD_SERVER_DEADLINE: lim = s.n_servers; break;
+        case AF_FIELD_CLIENT_TIMEOUT: lim = 1; break;
         default: return e->fail(AF_ERR_INVALID, "sweep: unknown field id");
         }
         if (i < 0 || i >= lim) return e->fail(AF_ERR_INVALID, "sweep: column index out of range");
@@ -603,6 +610,7 @@ int af_sweep_upload(af_engine* e, const AfSweep* sw, uint64_t first_replica) {
             case AF_FIELD_SERVER_CPU_CORES: case AF_FIELD_SERVER_RAM_MB: ok = ok && v >= 1.0 && v <= 2147483647.0; break;
             case AF_FIELD_ENDPOINT_RAM: ok = ok && v >= 0.0 && v <= 2147483647.0; break;
             case AF_FIELD_SERVER_MAX_IN_SERVICE: break;                         // afh::admission_sweep_fits
+            case AF_FIELD_SERVER_DEADLINE: case AF_FIELD_CLIENT_TIMEOUT: break;  // afh::deadline_sweep_fits
             case AF_FIELD_EDGE_MEAN: {
                 const int d = s.edges[sw->columns[c].index].dist;
                 ok = ok && (v >= 0.0 || d == AF_DIST_LOG_NORMAL || d == AF_DIST_NORMAL);
@@ -627,7 +635,8 @@ int af_sweep_upload(af_engine* e, const AfSweep* sw, uint64_t first_replica) {
     {
         std::string why;
         if (!afh::lb_sweep_fits(s, sw->columns, sw->n_columns, sw->values, sw->n_rows, why)
-            || !afh::admission_sweep_fits(sw->columns, sw->n_columns, sw->values, sw->n_rows, why)) return e->fail(AF_ERR_INVALID, why);
+            || !afh::admission_sweep_fits(sw->columns, sw->n_columns, sw->values, sw->n_rows, why)
+            || !afh::deadline_sweep_fits(sw->columns, sw->n_columns, sw->values, sw->n_rows, why)) return e->fail(AF_ERR_INVALID, why);
     }
     e->h_sweep_cols.assign(sw->columns, sw->columns + sw->n_columns);
     e->h_sweep_alias = aflh::column_aliases(sw->values, sw->n_rows, sw->n_columns);
@@ -1016,6 +1025,7 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
         if ((rc = upload_vec(e, e->d_l_outages, e->lt.outages, "lane tables"))) return rc;
         if ((rc = upload_vec(e, e->d_l_lb, e->lt.lb, "lane tables"))) return rc;
         if ((rc = upload_vec(e, e->d_l_cols, e->lt.cols, "lane tables"))) return rc;
+        if ((rc = upload_vec(e, e->d_l_dl, e->lt.dl_base, "lane tables"))) return rc;
         AF_CUDA(e, e->d_counter2.ensure(8), "work counter");
         AF_CUDA(e, e->d_redo_list.ensure(n * 4), "flagged-replica list");
         AF_CUDA(e, e->d_redo_count.ensure(4), "flagged-replica count");
@@ -1048,6 +1058,11 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
     if (occ) AF_CUDA(e, e->d_occ.ensure(n * (uint64_t)occ_cols * 8), "occupancy rows");
     const bool adm = afh::admission_launch(e->sc, e->h_sweep_cols.data(), e->sweep_cols);
     if (adm) AF_CUDA(e, e->d_rejected.ensure(n * (uint64_t)L.n_servers * 4), "rejection counts");
+    const bool dl = afh::deadline_launch(e->sc, e->h_sweep_cols.data(), e->sweep_cols);
+    if (dl) {
+        AF_CUDA(e, e->d_expired.ensure(n * (uint64_t)L.n_servers * 4), "expiry counts");
+        AF_CUDA(e, e->d_late.ensure(n * 4), "late counts");
+    }
     // pull order: the first pass runs `workers` replicas at once (lanes, or warps without the thread-per-replica pass)
     const uint64_t workers = lane ? lgrid * (uint64_t)lane_warps * 32ull : warp_slots;
     const uint64_t wave = workers < n ? workers : n;
@@ -1092,6 +1107,9 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
     G.redo_count = redo ? (const uint32_t*)e->d_redo_count.p : nullptr;
     G.seed = seed; G.replica_begin = begin; G.n_replicas = n;
     band.server_rejected = adm ? (uint32_t*)e->d_rejected.p : nullptr;
+    band.server_expired = dl ? (uint32_t*)e->d_expired.p : nullptr;
+    band.late = dl ? (uint32_t*)e->d_late.p : nullptr;
+    band.client_timeout = e->sc.client_timeout;
     if (occ) { band.occ = (uint64_t*)e->d_occ.p; band.occ_scale = ldexp(1.0, e->occ_opt.frac_bits); }
     afc::TimelineArgs tl = {};
     if (e->tl_rows) {
@@ -1150,6 +1168,8 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
         }
         C.stream_of = rs.stream_of; C.stream_first = rs.first; C.stream_rows = rs.rows;
         C.server_rejected = band.server_rejected;
+        C.dl_base = C.dl ? (const double*)e->d_l_dl.p : nullptr;
+        C.server_expired = band.server_expired; C.late = band.late;
     }
 
     // ---- enqueue ---------------------------------------------------------------------------------------------------
@@ -1169,6 +1189,10 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
     if (lat) AF_CUDA(e, cudaMemsetAsync(e->d_lat.p, 0, lat_words * 8, e->stream), "memset latency band rows");
     if (dist) AF_CUDA(e, cudaMemsetAsync(e->d_dist.p, 0, dist_words * 4, e->stream), "memset distribution band rows");
     if (adm) AF_CUDA(e, cudaMemsetAsync(e->d_rejected.p, 0, n * (uint64_t)L.n_servers * 4, e->stream), "memset rejection counts");
+    if (dl) {
+        AF_CUDA(e, cudaMemsetAsync(e->d_expired.p, 0, n * (uint64_t)L.n_servers * 4, e->stream), "memset expiry counts");
+        AF_CUDA(e, cudaMemsetAsync(e->d_late.p, 0, n * 4, e->stream), "memset late counts");
+    }
     {   // the pull order: (work, local index) heaviest first; then the first wave grouped by estimate
         uint32_t* key = (uint32_t*)e->d_okey.p; uint32_t* idx = (uint32_t*)e->d_oidx.p; uint32_t* order = (uint32_t*)e->d_order.p;
         uint64_t* key64 = (uint64_t*)e->d_okey64.p;
@@ -1225,7 +1249,7 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
         e->launches += 1;
     }
     AF_CUDA(e, cudaEventRecord(e->ev_end, e->stream), "event");
-    e->last_n = n; e->ran = true; e->timing_valid = false; e->last_adm = adm;
+    e->last_n = n; e->ran = true; e->timing_valid = false; e->last_adm = adm; e->last_dl = dl;
     e->last_lane = lane; e->last_warp = warp; e->last_lean = lean; e->last_lane_warps = lane_warps;
     e->last_bands = bands; e->last_band_groups = e->band_groups; e->last_band_ticks = (uint32_t)band_ticks;
     e->last_band_stride = band_stride;
@@ -1335,6 +1359,20 @@ int af_fetch_server_rejected(af_engine* e, uint32_t* out, uint64_t n) {
         return AF_OK;
     }
     return fetch(e, out, e->d_rejected, n * (uint64_t)e->L.n_servers * 4, n, "rejection counts D2H");
+}
+int af_fetch_server_expired(af_engine* e, uint32_t* out, uint64_t n) {
+    if (e && e->ran && out && n == e->last_n && !e->last_dl) {       // no deadline anywhere: nothing was dropped
+        memset(out, 0, n * (uint64_t)e->L.n_servers * 4);
+        return AF_OK;
+    }
+    return fetch(e, out, e->d_expired, n * (uint64_t)e->L.n_servers * 4, n, "expiry counts D2H");
+}
+int af_fetch_late(af_engine* e, uint32_t* out, uint64_t n) {
+    if (e && e->ran && out && n == e->last_n && !e->last_dl) {       // no timeout anywhere: nothing was late
+        memset(out, 0, n * 4);
+        return AF_OK;
+    }
+    return fetch(e, out, e->d_late, n * 4, n, "late counts D2H");
 }
 int af_fetch_histograms(af_engine* e, uint32_t* out, uint64_t n) {
     if (e && e->ran && !e->L.collect_hist) return e->fail(AF_ERR_STATE, "histograms were not collected");

@@ -61,7 +61,10 @@ inline bool validate(const AfScenario& s, std::string& err) {
         AF_CHECK(v.n_endpoints >= 1 && v.endpoint_begin >= 0 && v.endpoint_begin + v.n_endpoints <= s.n_endpoints,
                  "server %d: endpoint range", i);
         AF_CHECK(v.max_in_service >= 0, "server %d: max_in_service=%d must be >= 0 (0 = no admission limit)", i, v.max_in_service);
+        AF_CHECK(isfinite(v.deadline) && v.deadline >= 0.0, "server %d: deadline=%g must be finite and >= 0 (0 = none)", i, v.deadline);
     }
+    AF_CHECK(isfinite(s.client_timeout) && s.client_timeout >= 0.0, "client_timeout=%g must be finite and >= 0 (0 = none)",
+             s.client_timeout);
     for (int i = 0; i < s.n_endpoints; ++i) {
         const AfEndpoint& p = s.endpoints[i];
         AF_CHECK(p.n_steps >= 0 && p.n_steps <= 255 && p.step_begin >= 0 && p.step_begin + p.n_steps <= s.n_steps,
@@ -130,6 +133,38 @@ inline bool admission_sweep_fits(const AfSweepColumn* cols, int32_t n_cols, cons
                 char b[200];
                 snprintf(b, sizeof b, "sweep: row %llu column %d (server_max_in_service, server %d): value %g is not an "
                          "integer in [0, 2^31)", (unsigned long long)r, c, cols[c].index, v);
+                err = b;
+                return false;
+            }
+        }
+    }
+    return true;
+}
+
+// Does a launch have a request deadline or a client timeout somewhere (DESIGN.md §3.13)?  A scenario value, or a sweep
+// column over AF_FIELD_SERVER_DEADLINE / AF_FIELD_CLIENT_TIMEOUT (even one of zeros): only such launches lay out the
+// kernels' deadline words and fill the expired / late outputs.
+inline bool deadline_launch(const AfScenario& s, const AfSweepColumn* cols, int32_t n_cols) {
+    if (s.client_timeout > 0.0) return true;
+    for (int32_t i = 0; i < s.n_servers; ++i) if (s.servers[i].deadline > 0.0) return true;
+    for (int32_t c = 0; c < n_cols; ++c)
+        if (cols[c].field == AF_FIELD_SERVER_DEADLINE || cols[c].field == AF_FIELD_CLIENT_TIMEOUT) return true;
+    return false;
+}
+
+// af_sweep_upload's check of the AF_FIELD_SERVER_DEADLINE / AF_FIELD_CLIENT_TIMEOUT columns: every value finite and
+// >= 0 (naming the row).  Index ranges are checked with the other fields'.
+inline bool deadline_sweep_fits(const AfSweepColumn* cols, int32_t n_cols, const double* vals, uint64_t n_rows, std::string& err) {
+    for (int32_t c = 0; c < n_cols; ++c) {
+        const int32_t f = cols[c].field;
+        if (f != AF_FIELD_SERVER_DEADLINE && f != AF_FIELD_CLIENT_TIMEOUT) continue;
+        for (uint64_t r = 0; r < n_rows; ++r) {
+            const double v = vals[r * (uint64_t)n_cols + (uint64_t)c];
+            if (!(v >= 0.0 && isfinite(v))) {                               // (NaN fails the first test)
+                char b[200];
+                snprintf(b, sizeof b, "sweep: row %llu column %d (%s %d): value %g is not a finite number of seconds >= 0",
+                         (unsigned long long)r, c, f == AF_FIELD_SERVER_DEADLINE ? "server_deadline, server" : "client_timeout, index",
+                         cols[c].index, v);
                 err = b;
                 return false;
             }

@@ -96,8 +96,9 @@ constexpr uint32_t SLOT_BITS = 20, AUX_BITS = 9;
 constexpr uint32_t SLOT_MASK = (1u << SLOT_BITS) - 1, AUX_MASK = (1u << AUX_BITS) - 1;
 AFL_IN uint32_t mk_payload(uint32_t kind, uint32_t aux, uint32_t slot) { return (kind << 29) | (aux << SLOT_BITS) | slot; }
 
-// ---- request record pack: hops[0:8) step[8:16) ep[16:28) core[28] io[29] wait[30] -------------
+// ---- request record pack: hops[0:8) step[8:16) ep[16:28) core[28] io[29] wait[30] expired[31] ---
 constexpr uint32_t PK_CORE = 1u << 28, PK_IO = 1u << 29, PK_WAIT = 1u << 30;
+constexpr uint32_t PK_EXPIRED = 1u << 31;    // past its server's deadline: the handler's tail runs, no forward (§3.13)
 AFL_IN uint32_t pk_hops(uint32_t p) { return p & 0xFFu; }
 AFL_IN uint32_t pk_step(uint32_t p) { return (p >> 8) & 0xFFu; }
 AFL_IN uint32_t pk_ep(uint32_t p) { return (p >> 16) & 0xFFFu; }
@@ -206,6 +207,14 @@ struct Cfg {
     // requests it shed, written to server_rejected[local * n_servers + s] at write-back
     int32_t adm, o32_adm, c_rej;
     uint32_t* server_rejected;
+    // request deadlines and the client timeout (DESIGN.md §3.13), laid out only when dl != 0 (aflh::Tables.dl): the
+    // 64-bit word o64_dl + s holds server s's deadline, o64_dl + n_servers the client timeout (+inf: none), from the
+    // scenario's dl_base[0 .. n_servers] (same order), then the sweep row.  The cold word c_exp + s counts the requests
+    // server s dropped, c_exp + n_servers the late completions, written to server_expired[local * n_servers + s] and
+    // late[local] at write-back
+    int32_t dl, o64_dl, c_exp, dl_pad;
+    const double* dl_base;
+    uint32_t* server_expired; uint32_t* late;
 };
 // Cfg.lb_algo of a launch that sweeps the load-balancer algorithm (AF_FIELD_LB_ALGORITHM; DESIGN.md §3.11): each replica
 // reads its own from the 32-bit word right after its LB order, o32_lb + n_lb_edges
@@ -457,6 +466,34 @@ AFL_IN bool adm_shed(const Mem& m, uint32_t sidx, uint32_t out_edge) {
     i32_st(m, w, budget - 1);
     return false;
 }
+// Request deadlines (Cfg.dl; DESIGN.md §3.13; the full build only -- aflh::lean_launch).  A request past its server's
+// deadline at a CPU step runs the tail of the handler with PK_EXPIRED set; where the handler would hand it to the
+// out-edge, its record is released instead and dl_abandon counts it.  It never sends, so it leaves service by giving its
+// admission back (adm_shed derives the requests in service from the out-edge's sends).
+AFL_COLD void dl_abandon(const Mem m, uint32_t sidx) {
+    c32_st(m, AFL_C.c_exp + (int32_t)sidx, c32_ld(m, AFL_C.c_exp + (int32_t)sidx) + 1u);
+    if (AFL_C.adm) {
+        const int32_t w = AFL_C.o32_adm + (int32_t)sidx;
+        const int32_t budget = i32_ld(m, w);
+        if (budget != ADM_FREE) i32_st(m, w, budget + 1);
+    }
+}
+// start_replica: every server's deadline and the client timeout from the scenario (+inf: none; a sweep row overrides
+// them after), no expiry and no late completion yet
+AFL_COLD void dl_start(const Mem m) {
+    for (int32_t i = 0; i <= AFL_C.n_servers; ++i) {
+        const double v = AFL_C.dl_base[i];
+        f64_st(m, AFL_C.o64_dl + i, v > 0.0 ? v : afr::u2d(INF_BITS));
+        c32_st(m, AFL_C.c_exp + i, 0);
+    }
+}
+// write_back: the expiries and late completions of the replica in output slot `local`
+AFL_COLD void dl_write_back(const Mem m, uint64_t local) {
+    for (int32_t i = 0; i < AFL_C.n_servers; ++i)
+        AFL_C.server_expired[local * (uint64_t)AFL_C.n_servers + (uint32_t)i] = c32_ld(m, AFL_C.c_exp + i);
+    AFL_C.late[local] = c32_ld(m, AFL_C.c_exp + AFL_C.n_servers);
+}
+
 // start_replica: every server's word from the scenario (a sweep row overrides it after), no rejection yet
 AFL_COLD void adm_start(const Mem m) {
     for (int32_t i = 0; i < AFL_C.n_servers; ++i) {
@@ -930,6 +967,9 @@ AFL_IN void complete(St& W, const Mem& m, uint32_t slot, double t0, uint32_t& la
         if (b < AFL_C.horizon_s) red_add(&AFL_C.thr[local * (uint64_t)AFL_C.horizon_s + (uint32_t)b], 1u);
     }
     if constexpr (!kLean) {              // (`if (!kLean && ...)` here moves the SASS of the full kernel)
+        // later than the client timeout (DESIGN.md §3.13): still a completion everywhere else
+        if (AFL_C.dl && lat > f64_ld(m, AFL_C.o64_dl + AFL_C.n_servers))
+            c32_st(m, AFL_C.c_exp + AFL_C.n_servers, c32_ld(m, AFL_C.c_exp + AFL_C.n_servers) + 1u);
         if (AFL_UNLIKELY(W.traced != 0)) {
             if ((int32_t)(done - 1) < AFL_C.trace_clock_cap) {
                 double* p = AFL_C.trace_clocks + (local * (uint64_t)AFL_C.trace_clock_cap + (done - 1)) * 2;
@@ -980,6 +1020,7 @@ AFL_IN void start_replica(St& W, const Mem& m, uint64_t local_index) {
         c32_st(m, sq_word((uint32_t)i, SQ_RAMQ_NEED), 0);
     }
     if (!kLean && C.adm) adm_start(m);
+    if (!kLean && C.dl) dl_start(m);
 #pragma unroll 1
     for (int32_t i = 0; i < C.n_servers + 2; ++i) {
         c32_st(m, ib_word((uint32_t)i, IB_HEAD), NIL); c32_st(m, ib_word((uint32_t)i, IB_TAIL), NIL); c32_st(m, ib_word((uint32_t)i, IB_PENDING), 1);
@@ -1001,6 +1042,12 @@ AFL_IN void start_replica(St& W, const Mem& m, uint64_t local_index) {
         if (col.slot >= 0) { f64_st(m, C.o64_row + col.slot, v); continue; }
         if (col.field == AF_FIELD_LB_ALGORITHM) { w32_st(m, C.o32_lb + C.n_lb_edges, (uint32_t)(int32_t)v); continue; }   // (base: the scenario's)
         if (!has_row || gen_field(col.field, v, W.users_mean, W.users_sigma, W.rate_per_user)) continue;
+        if constexpr (!kLean) {          // (cases of the switch below would move the SASS of the lean kernel)
+            if (col.field == AF_FIELD_SERVER_DEADLINE || col.field == AF_FIELD_CLIENT_TIMEOUT) {
+                f64_st(m, C.o64_dl + (col.field == AF_FIELD_SERVER_DEADLINE ? col.index : C.n_servers), v > 0.0 ? v : afr::u2d(INF_BITS));
+                continue;
+            }
+        }
         switch (col.field) {
         case AF_FIELD_SERVER_CPU_CORES: i32_st(m, sv_word((uint32_t)col.index, SV_CPU_FREE), (int32_t)v); break;
         case AF_FIELD_SERVER_RAM_MB: i32_st(m, sv_word((uint32_t)col.index, SV_RAM_FREE), (int32_t)v); break;
@@ -1048,6 +1095,7 @@ AFL_IN void write_back(St& W, const Mem& m) {
         C.samp_max[local * (uint64_t)C.n_series + (uint32_t)j] = mx;
     }
     if (!kLean && C.adm) adm_write_back(m, local);
+    if (!kLean && C.dl) dl_write_back(m, local);
     AfReplicaStats st;
     st.n_events = W.n_events; st.generated = W.generated; st.completed = W.completed;
     st.flags = W.flags; st.n_ticks = W.n_ticks; st.peak_events = W.peak_ev; st.peak_requests = W.peak_rq;
@@ -1292,6 +1340,9 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                 ram_walk<kOcc>(W, m, sidx);
                 edge = ro(C.servers + sidx).out_edge;
                 act = A_SEND;
+                if constexpr (!kLean) {                        // past its deadline: released, not forwarded
+                    if (pack & PK_EXPIRED) { act = A_NONE; rq_release(W, m, slot); dl_abandon(m, sidx); }
+                }
             }
         }
         AFL_SYNC();
@@ -1401,6 +1452,15 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                                 break;
                             }
                         }
+                        // the request holds a core: past its server's deadline it abandons -- the tail of the handler
+                        // as it stands (core, then RAM), no forward (DESIGN.md §3.13)
+                        // (`if constexpr`: the lean kernel's SASS stays what it was)
+                        if constexpr (!kLean) {
+                            if (C.dl && AFL_UNLIKELY(W.now - t0 > f64_ld(m, C.o64_dl + (int32_t)sidx))) {
+                                pack = (pack & ~0xFF00u) | (ep.n_steps << 8) | PK_EXPIRED;
+                                continue;
+                            }
+                        }
                     } else {
                         if (pack & PK_CORE) {                // yield CPU.put(1): level rises NOW
                             i32_st(m, sv_word(sidx, SV_CPU_FREE), i32_ld(m, sv_word(sidx, SV_CPU_FREE)) + 1);
@@ -1442,6 +1502,13 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                 }
                 edge = ro(C.servers + sidx).out_edge;
                 act = A_SEND;
+                if constexpr (!kLean) {                      // past its deadline: released, not forwarded (the pack
+                    if (pack & PK_EXPIRED) {                 // store below lands in the freed slot, which no one reads)
+                        act = A_NONE;
+                        rq_release(W, m, slot);
+                        dl_abandon(m, sidx);
+                    }
+                }
                 break;
             }
             if (act != A_SEND) rq_pack_set(W, m, slot, pack);   // the request yields here: its record goes back (SEND stores its own)

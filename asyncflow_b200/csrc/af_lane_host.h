@@ -16,6 +16,10 @@ struct Tables {
     int32_t n_row = 0;
     int32_t lb_algo_word = 0;      // 1: a column sweeps the LB algorithm (a 32-bit word per lane after the LB order)
     int32_t adm = 0;               // 1: an admission limit somewhere (afh::admission_launch): a 32-bit word per server and lane
+    // 1: a deadline or a client timeout somewhere (afh::deadline_launch): n_servers + 1 64-bit words per lane, from
+    // dl_base (the scenario's deadline of each server, then its client timeout; 0: none)
+    int32_t dl = 0;
+    std::vector<double> dl_base;
 };
 
 // Scenario (+ the sweep's columns) -> the kernel's read-only tables.  A column over a field the kernel
@@ -37,7 +41,9 @@ inline bool build_tables(const AfScenario& s, const AfSweepColumn* cols, int32_t
         v.cpu_cores = a.cpu_cores; v.ram_mb = a.ram_mb; v.out_edge = (uint32_t)a.out_edge;
         v.ep_begin = (uint32_t)a.endpoint_begin; v.n_ep = (uint32_t)a.n_endpoints; v.c_cores = v.c_ram = -1; v.max_in_service = a.max_in_service;
         if (a.max_in_service > 0) t.adm = 1;
+        if (a.deadline > 0.0) t.dl = 1;
     }
+    if (s.client_timeout > 0.0) t.dl = 1;
     t.endpoints.resize((size_t)s.n_endpoints);
     for (int i = 0; i < s.n_endpoints; ++i) {
         const AfEndpoint& a = s.endpoints[i]; afl::EndpointP& p = t.endpoints[(size_t)i];
@@ -79,12 +85,19 @@ inline bool build_tables(const AfScenario& s, const AfSweepColumn* cols, int32_t
         case AF_FIELD_LB_COVERED: k.base = 1.0; break;
         case AF_FIELD_LB_ALGORITHM: k.base = s.lb_algo; t.lb_algo_word = 1; break;
         case AF_FIELD_SERVER_MAX_IN_SERVICE: k.base = s.servers[i].max_in_service; t.adm = 1; break;
+        case AF_FIELD_SERVER_DEADLINE: k.base = s.servers[i].deadline; t.dl = 1; break;
+        case AF_FIELD_CLIENT_TIMEOUT: k.base = s.client_timeout; t.dl = 1; break;
         default: err = "sweep: unknown field id"; return false;
         }
 #undef AFLH_SLOT
     }
     if (n_row > 32000) { err = "sweep: too many looked-up columns for the lane engine"; return false; }
     t.n_row = n_row;
+    if (t.dl) {
+        t.dl_base.resize((size_t)s.n_servers + 1);
+        for (int i = 0; i < s.n_servers; ++i) t.dl_base[(size_t)i] = s.servers[i].deadline;
+        t.dl_base[(size_t)s.n_servers] = s.client_timeout;
+    }
     return true;
 }
 
@@ -198,7 +211,7 @@ constexpr int32_t LANE_REQUEST_CAPACITY = 2048;
 // LB order, the gauges' dirty bits (32-bit).  (The gauges' sums / maxima and the send counters are write-only: global tier.)
 inline int32_t fixed_lane_bytes(const AfScenario& s, const Tables& t) {
     const int32_t n_series = 3 * s.n_servers + s.n_edges;
-    const int32_t fix64 = (s.n_spike_marks > 0 ? s.n_edges : 0) + t.n_row;
+    const int32_t fix64 = (s.n_spike_marks > 0 ? s.n_edges : 0) + t.n_row + t.dl * (s.n_servers + 1);
     const int32_t fix32 = s.n_edges + afl::SV_WORDS * s.n_servers + s.n_lb_edges + t.lb_algo_word + t.adm * s.n_servers + (n_series + 31) / 32;
     return 8 * fix64 + 4 * fix32;
 }
@@ -213,15 +226,20 @@ inline void pool_split(const afl::Cfg& C, int32_t need, int32_t& ev_s, int32_t& 
 }
 
 // Does a launch qualify for the lean lane kernel (run_lane<*, *, true>)?  No spikes, no outages, no traced replica,
-// every edge normal or exponential, every server with one endpoint, and no admission limit (a scenario limit or an
+// every edge normal or exponential, every server with one endpoint, no admission limit (a scenario limit or an
 // AF_FIELD_SERVER_MAX_IN_SERVICE column in `cols`: the lean loop leaves the check out, and the loop `bench.py` runs keeps
-// the instructions it had).  No other sweep column can change any of these.
+// the instructions it had), and no deadline or client timeout (likewise; AF_FIELD_SERVER_DEADLINE /
+// AF_FIELD_CLIENT_TIMEOUT).  No other sweep column can change any of these.
 inline bool lean_launch(const AfScenario& s, int32_t trace_replicas, const AfSweepColumn* cols = nullptr, int32_t n_cols = 0) {
     if (s.n_spike_marks > 0 || s.n_outage_marks > 0 || trace_replicas > 0) return false;
     for (int i = 0; i < s.n_servers; ++i)
         if (s.servers[i].max_in_service > 0) return false;
+    if (s.client_timeout > 0.0) return false;
+    for (int i = 0; i < s.n_servers; ++i)
+        if (s.servers[i].deadline > 0.0) return false;
     for (int32_t c = 0; c < n_cols; ++c)
-        if (cols[c].field == AF_FIELD_SERVER_MAX_IN_SERVICE) return false;
+        if (cols[c].field == AF_FIELD_SERVER_MAX_IN_SERVICE || cols[c].field == AF_FIELD_SERVER_DEADLINE
+            || cols[c].field == AF_FIELD_CLIENT_TIMEOUT) return false;
     for (int i = 0; i < s.n_edges; ++i)
         if (s.edges[i].dist != AF_DIST_NORMAL && s.edges[i].dist != AF_DIST_EXPONENTIAL) return false;
     for (int i = 0; i < s.n_servers; ++i)
@@ -252,7 +270,7 @@ inline bool make_cfg(const AfScenario& s, const AfOptions& o, const Tables& t, i
     int32_t rq_total = o.request_capacity > 0 ? o.request_capacity : LANE_REQUEST_CAPACITY;
     if (rq_total > (int32_t)afl::SLOT_MASK) rq_total = (int32_t)afl::SLOT_MASK;
     // fixed part of a lane's shared memory
-    const int32_t fix64 = (C.n_spike > 0 ? C.n_edges : 0) + C.n_row;
+    const int32_t fix64 = (C.n_spike > 0 ? C.n_edges : 0) + C.n_row + t.dl * (C.n_servers + 1);
     C.n_dirty = (C.n_series + 31) / 32;
     const int32_t fix32 = C.n_edges + afl::SV_WORDS * C.n_servers + C.n_lb_edges + t.lb_algo_word + t.adm * C.n_servers + C.n_dirty;
     int32_t nq_s = 0;                                // zero-delay items: ties only -- the ring starts in the global tier
@@ -279,6 +297,8 @@ inline bool make_cfg(const AfScenario& s, const AfOptions& o, const Tables& t, i
     C.o64_nq = e; e += nq_s;
     C.o64_spike = e; e += C.n_spike > 0 ? C.n_edges : 0;
     C.o64_row = e; e += C.n_row;
+    C.dl = t.dl; C.o64_dl = e; e += t.dl * (C.n_servers + 1);
+    C.dl_base = t.dl ? t.dl_base.data() : nullptr;   // the host copy (the twin runs on it); af_run points at the device's
     C.n64 = e;
     int32_t w = 0;
     C.o32_conn = w; w += C.n_edges;
@@ -300,7 +320,8 @@ inline bool make_cfg(const AfScenario& s, const AfOptions& o, const Tables& t, i
     C.g32_cold = hcount;
     C.c_srvq = 0; C.c_inbox = C.c_srvq + afl::SQ_WORDS * C.n_servers; C.c_drop = C.c_inbox + afl::IB_WORDS * (C.n_servers + 2);
     C.c_rej = C.c_drop + C.n_edges;
-    hcount += C.c_rej + t.adm * C.n_servers;
+    C.c_exp = C.c_rej + t.adm * C.n_servers;
+    hcount += C.c_exp + t.dl * (C.n_servers + 1);
     C.gi_smax = hcount; hcount += C.n_series;
     C.gi_sent = hcount; hcount += C.n_edges;
     C.gn32 = hcount;

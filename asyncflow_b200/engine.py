@@ -160,6 +160,18 @@ class Engine:
         self._check(self._lib.af_fetch_server_rejected(self._h, out.ctypes.data, self._n), "af_fetch_server_rejected")
         return out
 
+    def server_expired(self, out: np.ndarray | None = None) -> np.ndarray:
+        """Requests each server dropped past its deadline, ``[n, n_servers]`` -- ``af_fetch_server_expired``."""
+        out = np.empty((self._n, self.flat.n_servers), dtype=np.uint32) if out is None else out
+        self._check(self._lib.af_fetch_server_expired(self._h, out.ctypes.data, self._n), "af_fetch_server_expired")
+        return out
+
+    def late(self, out: np.ndarray | None = None) -> np.ndarray:
+        """Completions later than the client timeout, ``[n]`` -- ``af_fetch_late``."""
+        out = np.empty(self._n, dtype=np.uint32) if out is None else out
+        self._check(self._lib.af_fetch_late(self._h, out.ctypes.data, self._n), "af_fetch_late")
+        return out
+
     def histograms(self) -> np.ndarray:
         out = np.empty((self._n, K.AF_HIST_BINS), dtype=np.uint32)
         self._check(self._lib.af_fetch_histograms(self._h, out.ctypes.data, self._n), "af_fetch_histograms")

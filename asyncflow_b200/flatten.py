@@ -100,6 +100,38 @@ def set_admission(flat: "FlatScenario", admission: dict[str, int] | None) -> Non
         flat.pod.servers[flat.server_ids.index(sid)].max_in_service = int(lim)
 
 
+def _seconds(x: Any) -> float:
+    """A deadline or a timeout as a float, NaN unless it is a finite number of seconds >= 0 (bools refused)."""
+    if isinstance(x, (bool, np.bool_)):
+        return np.nan
+    try:
+        v = float(x)
+    except (TypeError, ValueError):
+        return np.nan
+    return v if np.isfinite(v) and v >= 0.0 else np.nan
+
+
+def set_deadlines(flat: "FlatScenario", deadlines: dict[str, float] | None, *, client_timeout: float | None = None) -> None:
+    """The scenario's request deadlines and client timeout (DESIGN.md §3.13), in seconds, 0 = none:
+    ``deadlines[server_id]`` (servers left out keep theirs) and ``client_timeout`` (``None``: kept).  ``KeyError`` for
+    an unknown server, ``ValueError`` for a value that is not a finite number >= 0."""
+    for sid, v in (deadlines or {}).items():
+        if sid not in flat.server_ids:
+            msg = f"deadlines: no server {sid!r} (servers: {list(flat.server_ids)})"
+            raise KeyError(msg)
+        d = _seconds(v)
+        if d != d:
+            msg = f"deadlines: server {sid!r}: deadline {v!r} is not a finite number of seconds >= 0"
+            raise ValueError(msg)
+        flat.pod.servers[flat.server_ids.index(sid)].deadline = d
+    if client_timeout is not None:
+        t = _seconds(client_timeout)
+        if t != t:
+            msg = f"client_timeout {client_timeout!r} is not a finite number of seconds >= 0"
+            raise ValueError(msg)
+        flat.pod.client_timeout = t
+
+
 def _rv(d: dict) -> tuple[str, float, float]:
     dist = _s(d.get("distribution") or "poisson")
     var = d.get("variance")
@@ -441,7 +473,8 @@ class SweepSpec:
     ``("event_start"|"event_end", event_id)`` (the ``t_start`` / ``t_end`` of a spike or an outage),
     ``("lb_covered", server_id)`` (1: behind the load balancer as in the scenario, 0: not; bools accepted) and
     ``("lb_algorithm",)`` (``"round_robin"`` or ``"least_connection"``, enum members or ``K.LB_*`` codes accepted) and
-    ``("server_max_in_service", server_id)`` (the server's admission limit, an integer >= 0, 0 = none; DESIGN.md §3.12).
+    ``("server_max_in_service", server_id)`` (the server's admission limit, an integer >= 0, 0 = none; DESIGN.md §3.12),
+    ``("server_deadline", server_id)`` and ``("client_timeout",)`` (seconds >= 0, 0 = none; DESIGN.md §3.13).
 
     A row that uncovers a server simulates the scenario without the load balancer's edge to it (:meth:`payload_for`):
     its round-robin order is the scenario's with that edge left out, and an outage of that server is a no-op.  The
@@ -466,6 +499,7 @@ class SweepSpec:
         keys = [tuple(sel) if not isinstance(sel, str) else (sel,) for sel in columns]
         arrays = [self._lb_values(flat, sel, v) if sel[0] in ("lb_covered", "lb_algorithm")
                   else self._limits(flat, sel, v) if sel[0] in K.ADMISSION_FIELDS
+                  else self._seconds(flat, sel, v) if sel[0] in K.DEADLINE_FIELDS
                   else np.ascontiguousarray(np.broadcast_to(np.asarray(v, dtype=np.float64), (self.n_replicas,)))
                   for sel, v in zip(keys, columns.values())]
         self.covered = self._covered(flat, keys, arrays)
@@ -482,7 +516,7 @@ class SweepSpec:
                     raise KeyError(msg)
                 self.selectors.append((sel, arr))       # carried by the rows' timelines, not by a column
                 continue
-            if name in ("users_mean", "users_sigma", "rate_per_user"):
+            if name in ("users_mean", "users_sigma", "rate_per_user", "client_timeout"):
                 targets = [0]
             elif name.startswith("edge_"):
                 targets = [flat.edge_ids.index(sel[1])]
@@ -506,7 +540,7 @@ class SweepSpec:
                 raise KeyError(msg)
             self.selectors.append((sel, arr))
             for t in targets:
-                cols.append(({**K.FIELDS, **K.LB_FIELDS, **K.ADMISSION_FIELDS}[name], t))
+                cols.append(({**K.FIELDS, **K.LB_FIELDS, **K.ADMISSION_FIELDS, **K.DEADLINE_FIELDS}[name], t))
                 vals.append(arr)
         self.n_columns = len(cols)
         self.values = (np.ascontiguousarray(np.stack(vals, axis=1)) if vals
@@ -564,6 +598,46 @@ class SweepSpec:
             raise ValueError(msg)
         return out
 
+    def _seconds(self, flat: FlatScenario, sel: tuple, v: Any) -> np.ndarray:
+        """A deadline or client-timeout column: finite seconds >= 0 (``KeyError`` / ``ValueError`` naming the row)."""
+        if sel[0] == "server_deadline" and (len(sel) != 2 or sel[1] not in flat.server_ids):
+            msg = f"sweep column {sel!r}: no server {sel[1] if len(sel) > 1 else None!r} (servers: {list(flat.server_ids)})"
+            raise KeyError(msg)
+        if sel[0] == "client_timeout" and len(sel) != 1:
+            msg = f"sweep column {sel!r}: the client timeout takes no index (('client_timeout',))"
+            raise KeyError(msg)
+        raw = np.broadcast_to(np.asarray(v, dtype=object), (self.n_replicas,))
+        out = np.array([_seconds(x) for x in raw], dtype=np.float64)
+        bad = np.isnan(out)
+        if bad.any():
+            r = int(np.flatnonzero(bad)[0])
+            msg = f"sweep row {r}: {sel!r} = {raw[r]!r}: a deadline or timeout is a finite number of seconds >= 0 (0: none)"
+            raise ValueError(msg)
+        return out
+
+    def deadlines_for(self, replica: int) -> tuple[dict[str, float], float | None]:
+        """Row ``replica``'s deadlines ``{server_id: seconds}`` and client timeout (``None`` without such a column) from
+        this spec's columns (zeros included)."""
+        dl = {sel[1]: float(arr[replica]) for sel, arr in self.selectors if sel[0] == "server_deadline"}
+        to = [float(arr[replica]) for sel, arr in self.selectors if sel[0] == "client_timeout"]
+        return dl, (to[-1] if to else None)
+
+    def _refuse_deadlines(self, replica: int, what: str) -> None:
+        dl, to = self.deadlines_for(replica)
+        set_ = {**{sid: v for sid, v in dl.items() if v}, **({"client_timeout": to} if to else {})}
+        if set_:
+            msg = (f"sweep row {replica} sets deadlines {set_}, which {what} cannot express; "
+                   "payload_and_overload() returns the payload with the deadlines, the timeout and the limits")
+            raise ValueError(msg)
+
+    def payload_and_overload(self, payload: Any, replica: int) -> tuple[dict, dict]:
+        """Row ``replica`` as the oracle takes it: the row's payload (:meth:`payload_for` without the overload columns)
+        and ``{"admission": {server_id: limit}, "deadline": {server_id: seconds}, "client_timeout": seconds | None}``
+        (0: none; ``None``: the scenario's).  The reference can express none of them."""
+        dl, to = self.deadlines_for(replica)
+        return self._payload(payload, replica), {"admission": self.admission_for(replica), "deadline": dl,
+                                                 "client_timeout": to}
+
     def admission_for(self, replica: int) -> dict[str, int]:
         """Row ``replica``'s admission limits ``{server_id: limit}`` from this spec's columns (zeros included)."""
         return {sel[1]: int(arr[replica]) for sel, arr in self.selectors if sel[0] in K.ADMISSION_FIELDS}
@@ -571,7 +645,9 @@ class SweepSpec:
     def payload_and_admission(self, payload: Any, replica: int) -> tuple[dict, dict[str, int]]:
         """Row ``replica`` as the oracle takes it: the row's payload (:meth:`payload_for` without the admission
         columns) and its admission limits, ``{server_id: limit}`` (0: none).  The reference cannot express a limit, so a
-        capped row has no payload of its own."""
+        capped row has no payload of its own.  A row with a deadline or a client timeout is refused (``ValueError``):
+        use :meth:`payload_and_overload`."""
+        self._refuse_deadlines(replica, "payload_and_admission()")
         return self._payload(payload, replica), self.admission_for(replica)
 
     def _covered(self, flat: FlatScenario, keys: list[tuple], arrays: list[np.ndarray]) -> np.ndarray | None:
@@ -684,9 +760,10 @@ class SweepSpec:
         ``GpuSimulationRunner``) simulates exactly what row ``replica`` of the sweep simulates;
         it is how a sweep point is handed back to the reference for inspection, and how the parity
         tests build the oracle's input.  ``payload`` is the base scenario the sweep was made from.
-        A row with an admission limit has no such payload (the reference has no limits): ``ValueError``; use
-        :meth:`payload_and_admission`.
+        A row with an admission limit, a deadline or a client timeout has no such payload (the reference has none of
+        them): ``ValueError``; use :meth:`payload_and_overload`.
         """
+        self._refuse_deadlines(replica, "a payload")
         capped = {sid: v for sid, v in self.admission_for(replica).items() if v}
         if capped:
             msg = (f"sweep row {replica} sets admission limits {capped}, which a payload cannot express; "

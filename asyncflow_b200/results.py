@@ -171,6 +171,8 @@ class ReplicaResults:
     n_events: int
     flags: int
     server_rejected: dict[str, int] = field(default_factory=dict)   # requests each server shed at its admission limit
+    server_expired: dict[str, int] = field(default_factory=dict)    # requests each server dropped past its deadline
+    late: int = 0                                                    # completions later than the client timeout
 
     # -- analyzer-compatible getters (metrics/analyzer.py:147-262) -------------
     def list_server_ids(self) -> list[str]:
@@ -300,6 +302,10 @@ class SweepResults:
         self.replica_begin = replica_begin
         # requests each server shed at its admission limit, [n, n_servers] u32 (zeros without limits; DESIGN.md §3.12)
         self.server_rejected = np.zeros((len(stats), flat.n_servers if flat is not None else 0), dtype=np.uint32)
+        # requests each server dropped past its deadline, [n, n_servers] u32, and completions later than the client
+        # timeout, [n] u32 (zeros without deadlines / a timeout; DESIGN.md §3.13).  Goodput: completed - late
+        self.server_expired = np.zeros_like(self.server_rejected)
+        self.late = np.zeros(len(stats), dtype=np.uint32)
         self.rows: np.ndarray | None = None      # sweep row of each result row (set by SweepRunner)
         self.streams: np.ndarray | None = None   # random stream of each result row (SweepRunner.stream_ids; set by collect)
         self.traced: list[ReplicaResults] = []    # full clocks + sampled series of the first `trace_replicas` replica ids
@@ -469,6 +475,8 @@ class SweepResults:
                            self.replica_begin)
         out.traced = self.traced
         out.server_rejected = self.server_rejected[index]
+        out.server_expired = self.server_expired[index]
+        out.late = self.late[index]
         out.streams = g(self.streams)
         out.band_count, out.band_sum, out.band_sumsq = self.band_count, self.band_sum, self.band_sumsq
         out.lat_window_s, out.lat_hist, out.lat_sum_hi, out.lat_sum_lo = (self.lat_window_s, self.lat_hist,
@@ -669,6 +677,8 @@ class SweepResults:
             np.concatenate([p.samp_max for p in parts]), cat([p.throughput for p in parts]),
             cat([p.histograms for p in parts]), f.replica_begin)
         out.server_rejected = np.concatenate([p.server_rejected for p in parts])
+        out.server_expired = np.concatenate([p.server_expired for p in parts])
+        out.late = np.concatenate([p.late for p in parts])
         if all(p.streams is not None for p in parts):
             out.streams = np.concatenate([p.streams for p in parts])
         if all(p.band_count is not None for p in parts):      # integer sums over disjoint replicas: they add exactly

@@ -38,7 +38,7 @@
 extern "C" {
 #endif
 
-#define AF_ABI_VERSION 10
+#define AF_ABI_VERSION 11
 
 typedef enum AfStatus {
     AF_OK = 0,
@@ -82,6 +82,8 @@ typedef struct AfServer {        /* schemas/topology/nodes.py:52-104 */
     int32_t n_endpoints;
     int32_t max_in_service;      /* admission limit: requests in service at once   *
                                   * (0 = no limit; see AF_FIELD_SERVER_MAX_IN_SERVICE) */
+    double deadline;             /* request deadline in seconds from creation      *
+                                  * (0 = none; see AF_FIELD_SERVER_DEADLINE)       */
 } AfServer;
 
 typedef struct AfEndpoint {      /* schemas/topology/endpoint.py:92-102 */
@@ -139,6 +141,8 @@ typedef struct AfScenario {
     const int32_t* lb_edges;     /* initial round-robin order (edge indices)       */
     const AfSpikeMark* spike_marks;
     const AfOutageMark* outage_marks;
+    double client_timeout;       /* the client counts a completion later than this  *
+                                  * as late (0 = none; AF_FIELD_CLIENT_TIMEOUT)     */
 } AfScenario;
 
 /* Per-replica overrides of scenario fields: the Monte-Carlo sweep
@@ -152,7 +156,9 @@ enum {
     AF_FIELD_LB_COVERED = 11,    /* index = position in lb_edges; 1 = behind the LB as in the scenario, 0 = not */
     AF_FIELD_LB_ALGORITHM = 12,  /* index 0; an AF_LB_* algorithm (round robin or least connections)           */
     AF_FIELD_SERVER_MAX_IN_SERVICE = 13,  /* index = server; an admission limit, 0 = none (AfServer.max_in_service) */
-    AF_FIELD_COUNT = 14
+    AF_FIELD_SERVER_DEADLINE = 14,  /* index = server; a request deadline in seconds, 0 = none (AfServer.deadline) */
+    AF_FIELD_CLIENT_TIMEOUT = 15,   /* index 0; the client's timeout in seconds, 0 = none (AfScenario.client_timeout) */
+    AF_FIELD_COUNT = 16
 };
 /* Load-balancer rows (DESIGN.md §3.11).  A replica whose row sets AF_FIELD_LB_COVERED of position k to 0 runs without
  * the LB edge lb_edges[k]: its round-robin order is lb_edges with the uncovered edges left out; the server and its other
@@ -169,6 +175,15 @@ enum {
  * No random number is drawn, so replicas sharing a stream see the same traffic whatever their limits.  Replicas without
  * a row keep the scenario's limits.  af_scenario_upload refuses a negative max_in_service; af_sweep_upload refuses an
  * index out of range and a value that is not an integer in [0, 2^31) (naming the row). */
+/* Request deadlines (DESIGN.md §3.13).  A request's age is now - t0, t0 the time the generator created it, so a deadline
+ * holds end to end across a chain of servers.  A server with a deadline D > 0 (AfServer.deadline, or the replica's
+ * AF_FIELD_SERVER_DEADLINE value) checks the age once per CPU step, once the request holds a core and before the step's
+ * timeout.  When now - t0 > D the request abandons: it releases its core and RAM as a finished handler does, in the same
+ * order, and is not handed to the out-edge; af_fetch_server_expired counts it (and it leaves service for the admission
+ * limit).  A request that never runs a CPU step there, or waits for RAM, is not checked until its first CPU step.
+ * The client timeout T > 0 (AfScenario.client_timeout or AF_FIELD_CLIENT_TIMEOUT) counts a completion with
+ * now - t0 > T in af_fetch_late; the completion counts everywhere else as before.  Neither draws a random number.
+ * af_scenario_upload and af_sweep_upload refuse negative, NaN and infinite values (the latter naming the row). */
 typedef struct AfSweepColumn { int32_t field; int32_t index; } AfSweepColumn;
 typedef struct AfSweep {
     int32_t n_columns;
@@ -295,6 +310,10 @@ int af_fetch_edge_counts(af_engine* e, uint32_t* sent, uint32_t* dropped, uint64
 int af_fetch_histograms(af_engine* e, uint32_t* out, uint64_t n);   /* [n][AF_HIST_BINS] */
 /* requests each server shed at its admission limit: [n][n_servers] (all 0 when the run had no limit) */
 int af_fetch_server_rejected(af_engine* e, uint32_t* out, uint64_t n);
+/* requests each server dropped past its deadline: [n][n_servers]; completions later than the client timeout: [n]
+ * (all 0 when the run had no deadline and no timeout) */
+int af_fetch_server_expired(af_engine* e, uint32_t* out, uint64_t n);
+int af_fetch_late(af_engine* e, uint32_t* out, uint64_t n);
 int af_fetch_throughput(af_engine* e, uint32_t* out, uint64_t n);   /* [n][horizon_s]    */
 /* sampled-metric aggregates over ticks: per replica, per series j:
  *   j <  3*n_servers : server j/3, metric j%3 in {ready_queue_len, event_loop_io_sleep, ram_in_use}
