@@ -11,7 +11,7 @@ from __future__ import annotations
 import ctypes as C
 from pathlib import Path
 
-AF_ABI_VERSION = 11
+AF_ABI_VERSION = 12
 AF_HIST_BINS = 4096
 AF_HIST_SUB_BITS = 7
 AF_HIST_MIN_EXP = -20
@@ -38,6 +38,10 @@ ADMISSION_FIELDS = {"server_max_in_service": 13}
 #: request deadlines (AF_FIELD_SERVER_DEADLINE, per server) and the client timeout (AF_FIELD_CLIENT_TIMEOUT), in seconds,
 #: 0 = none.  Kept apart from FIELDS for the same reason (DESIGN.md §3.13).
 DEADLINE_FIELDS = {"server_deadline": 14, "client_timeout": 15}
+#: rate limits (DESIGN.md §3.14): a server's (AF_FIELD_SERVER_RATE / AF_FIELD_SERVER_BURST, per server) and the load
+#: balancer's (AF_FIELD_LB_RATE / AF_FIELD_LB_BURST), a rate in requests per second (0 = none) and a burst >= 1.  Kept
+#: apart from FIELDS for the same reason.
+RATE_FIELDS = {"server_rate": 16, "server_burst": 17, "lb_rate": 18, "lb_burst": 19}
 FLAG_EVENT_OVERFLOW, FLAG_REQUEST_OVERFLOW, FLAG_TRACE_TRUNCATED, FLAG_NOWQ_OVERFLOW, FLAG_LB_EMPTY = 1, 2, 4, 8, 16
 MODE_AUTO, MODE_WARP, MODE_LANE, MODE_TWO_PASS = 0, 1, 2, 3
 SELFTEST_EDGE, SELFTEST_GEN_UNIFORM, SELFTEST_GEN_USERS, SELFTEST_ENDPOINT = 0, 1, 2, 3
@@ -54,7 +58,7 @@ class AfEdge(C.Structure):
 class AfServer(C.Structure):
     _fields_ = [("cpu_cores", C.c_int32), ("ram_mb", C.c_int32), ("out_edge", C.c_int32),
                 ("endpoint_begin", C.c_int32), ("n_endpoints", C.c_int32), ("max_in_service", C.c_int32),
-                ("deadline", C.c_double)]
+                ("deadline", C.c_double), ("rate_limit", C.c_double), ("burst", C.c_int32), ("reserved", C.c_int32)]
 
 
 class AfEndpoint(C.Structure):
@@ -88,6 +92,7 @@ class AfScenario(C.Structure):
         ("endpoints", C.POINTER(AfEndpoint)), ("steps", C.POINTER(AfStep)),
         ("lb_edges", C.POINTER(C.c_int32)), ("spike_marks", C.POINTER(AfSpikeMark)),
         ("outage_marks", C.POINTER(AfOutageMark)), ("client_timeout", C.c_double),
+        ("lb_rate_limit", C.c_double), ("lb_burst", C.c_int32), ("reserved2", C.c_int32),
     ]
 
 
@@ -160,6 +165,7 @@ EXPORTS = [
     "af_selftest_rng", "af_bands_upload", "af_fetch_bands", "af_bands_configure", "af_fetch_latency_bands",
     "af_dist_bands_configure", "af_fetch_dist_bands", "af_occupancy_configure", "af_fetch_occupancy",
     "af_timeline_upload", "af_streams_upload", "af_fetch_server_rejected", "af_fetch_server_expired", "af_fetch_late",
+    "af_fetch_throttled",
 ]
 
 _lib = None
@@ -200,6 +206,7 @@ def load() -> C.CDLL:
     lib.af_fetch_server_rejected.argtypes = [vp, vp, u64]
     lib.af_fetch_server_expired.argtypes = [vp, vp, u64]
     lib.af_fetch_late.argtypes = [vp, vp, u64]
+    lib.af_fetch_throttled.argtypes = [vp, vp, u64]
     lib.af_fetch_throughput.argtypes = [vp, vp, u64]
     lib.af_fetch_sampled.argtypes = [vp, vp, vp, u64]
     lib.af_fetch_trace_clocks.argtypes = [vp, u64, vp, u64, C.POINTER(u64)]

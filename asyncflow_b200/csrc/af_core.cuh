@@ -147,6 +147,9 @@ struct StepS { double dur; uint32_t kind, pad; };                   // 16 B
 struct SpikeS { double fire, delta; uint32_t edge, pad; };           // 24 B
 struct OutageS { double fire; int32_t lb_edge, down; };              // 16 B
 struct InboxS { uint32_t head, tail, pending, pad; };                // 16 B: a node's Store + its consumer's pending get()
+// a server's rate limit (DESIGN.md §3.14; tbl_rate): its GCRA bucket's theoretical arrival time, tau and tolerance L
+// (tau = 0: no limit), and the requests it throttled
+struct RateS { double tat, tau, lim; uint32_t throttled, pad; };     // 32 B
 
 // The replica's scalar state: one per warp, at the start of the warp's workspace.
 struct State {
@@ -197,6 +200,8 @@ struct State {
     // client timeout (DESIGN.md §3.13; +inf: none) and the completions later than it
     double timeout;
     uint32_t late, late_pad;
+    // the load balancer's rate limit and the requests it throttled (DESIGN.md §3.14)
+    RateS lb_rl;
 };
 
 // Everything the kernel needs to know about sizes; built on the host.
@@ -244,6 +249,11 @@ struct BandArgs {
     // timeout, [n_replicas] u32 (nullptr: the launch has neither; DESIGN.md §3.13)
     uint32_t* server_expired; uint32_t* late;
     double client_timeout;         // the scenario's (0: none)
+    // requests each site throttled at its rate limit, [n_replicas][n_servers + 1] u32, column n_servers the load
+    // balancer (nullptr: the launch has no rate limit; DESIGN.md §3.14), and the scenario's LB rate (0: none) and burst
+    uint32_t* throttled;
+    double lb_rate;
+    int32_t lb_burst, rl_pad;
 };
 
 // Per-replica timelines of a launch (af_sim_kernel's parameter; rows == 0: none): replica first + r, r < rows, copies its
@@ -282,7 +292,9 @@ inline void layout_finalize(Layout& L) {
     L.off_samp_max = o; o += 4 * L.n_series;
     L.off_lb = o;       o += 4 * L.n_lb_edges;
     o = align_up(o, 8) + 8 * L.n_servers;  // each server's deadline (tbl_deadline: no Layout field, so that no
-    L.warp_bytes = align_up(o, 16);         // __constant__ offset of the lane kernel's moves)
+                                            // __constant__ offset of the lane kernel's moves)
+    o += 32 * L.n_servers;                  // each server's rate limit (tbl_rate; likewise)
+    L.warp_bytes = align_up(o, 16);
 }
 
 // Device-global pointers (read-only scenario, sweep rows, spill tiers, outputs).
@@ -341,6 +353,11 @@ AF_TBL(tbl_samp_max, uint32_t, off_samp_max)
 // each server's deadline in seconds (+inf: none; DESIGN.md §3.13), f64, right after the LB order
 AF_IN double* tbl_deadline(State& W) {
     return reinterpret_cast<double*>(reinterpret_cast<unsigned char*>(&W) + align_up(AF_L.off_lb + 4 * AF_L.n_lb_edges, 8));
+}
+// each server's rate limit (RateS; DESIGN.md §3.14), right after the deadlines
+AF_IN RateS* tbl_rate(State& W) {
+    return reinterpret_cast<RateS*>(reinterpret_cast<unsigned char*>(&W) + align_up(AF_L.off_lb + 4 * AF_L.n_lb_edges, 8)
+                                    + 8 * AF_L.n_servers);
 }
 AF_TBL(tbl_nq, uint64_t, off_nq)
 AF_TBL(tbl_inbox, InboxS, off_inbox)
@@ -779,10 +796,21 @@ AF_IN void on_cpu_put(State& W, uint32_t slot, uint32_t sidx) {
     run_steps(W, slot, sidx, r.rid, r.pack & ~PK_CORE);   // core_locked = False; same step again
 }
 
+// A site's process takes a request at W.now: true when its rate limit R throttles it (counted), else it spends a token
+// (afr::rl_pass; DESIGN.md §3.14).  Out of line: the check is off the path of launches without a limit.
+AF_FN bool rl_throttle(State& W, RateS& R) {
+    double tat = R.tat;
+    if (afr::rl_pass(tat, W.now, R.tau, R.lim)) { R.tat = tat; return false; }
+    R.throttled += 1;
+    return true;
+}
+
 // ServerRuntime._dispatcher resumed with `slot` (server.py:303-313), then the head of
 // _handle_request (server.py:88-149), which runs as an URGENT Initialize right after
 AF_IN void server_got(State& W, uint32_t slot, uint32_t sidx, const ReqRec& r) {
     consumer_get(W, NODE_SERVER0 + sidx);            // the dispatcher loops back to get() first
+    // throttled at its rate limit, before the admission limit (§3.14): gone as a shed request is
+    if (AF_UNLIKELY(tbl_rate(W)[sidx].tau != 0.0) && rl_throttle(W, tbl_rate(W)[sidx])) { rq_release(W, slot); return; }
     ServerS& S = tbl_server(W)[sidx];
     if (AF_UNLIKELY(S.adm_left == 0)) {              // at its admission limit: shed at the door, no handler
         S.rejected += 1;
@@ -884,6 +912,11 @@ AF_FN void node_got(State& W, uint32_t node, uint32_t slot, double t0, uint32_t 
         return;
     }
     rq_set_pack(W, slot, r.pack);
+    if (AF_UNLIKELY(W.lb_rl.tau != 0.0) && rl_throttle(W, W.lb_rl)) {   // throttled at the LB's rate limit: gone
+        consumer_get(W, NODE_LB);                                          // before the pick (§3.14)
+        rq_release(W, slot);
+        return;
+    }
     uint32_t* lb = tbl_lb(W);
     const int32_t n = W.lb_n;
     // every covered server is down: the reference dies here (StopIteration inside round_robin); the replica
@@ -1141,7 +1174,24 @@ AF_IN void bind(State& W, unsigned char* ws, uint64_t warp_slot) {
     W.sp_rq_next = AF_G.spill_rq_next + warp_slot * rq_sp;
 }
 
+// a site's rate and burst -> its tau and tolerance L (afr::rl_params; a rate of 0: no limit, tau = 0; a burst below 1
+// reads as 1)
+AF_IN void rl_finish(double& tau, double& lim) {
+    const double rate = tau, burst = lim;
+    tau = 0.0; lim = 0.0;
+    if (rate > 0.0) afr::rl_params(rate, burst < 1.0 ? 1.0 : burst, tau, lim);
+}
+
+// the requests each site of the replica throttled, to its output row `out` ([n_servers + 1], the LB last)
+AF_FN void rl_write_back(State& W, uint32_t* out) {
+    AF_SHARED(&W);
+    for (int32_t i = lane_id(); i < AF_L.n_servers; i += WARP) out[i] = tbl_rate(W)[i].throttled;
+    if (lane_id() == 0) out[AF_L.n_servers] = W.lb_rl.throttled;
+    w_sync();
+}
+
 // `spikes` / `outages`: the replica's mark tables (its timeline row, or the scenario's)
+// The caller has set W.lb_rl.tau / .lim to the scenario's LB rate and burst (rl_finish turns them into tau and L).
 AF_FN void load_params(State& W, const AfSpikeMark* spikes, const AfOutageMark* outages, double client_timeout) {
     AF_SHARED(&W);
     const int lane = lane_id();
@@ -1164,6 +1214,8 @@ AF_FN void load_params(State& W, const AfSpikeMark* spikes, const AfOutageMark* 
         s.ramq_head_need = 0; s.adm_left = a.max_in_service > 0 ? (uint32_t)a.max_in_service : 0xFFFFFFFFu; s.rejected = 0;
         s.expired = 0;
         tbl_deadline(W)[i] = a.deadline > 0.0 ? a.deadline : INF_DEADLINE;
+        RateS q; q.tat = 0.0; q.tau = a.rate_limit; q.lim = (double)a.burst; q.throttled = 0; q.pad = 0;   // (rl_finish)
+        tbl_rate(W)[i] = q;
         tbl_server(W)[i] = s;
     }
 #pragma unroll 1
@@ -1202,6 +1254,7 @@ AF_FN void load_params(State& W, const AfSpikeMark* spikes, const AfOutageMark* 
     W.users_mean = AF_L.users_mean; W.users_sigma = AF_L.users_sigma; W.rate_per_user = AF_L.rate_per_user;
     W.lb_algo = AF_L.lb_algo;
     W.timeout = client_timeout > 0.0 ? client_timeout : INF_DEADLINE; W.late = 0; W.late_pad = 0;
+    W.lb_rl.tat = 0.0; W.lb_rl.throttled = 0; W.lb_rl.pad = 0;
     // sweep overrides of this replica (uniform: every lane applies every column)
     const uint64_t replica = AF_G.replica_begin + W.local;     // (W.replica is its stream)
     if (AF_L.n_sweep_cols > 0 && replica >= AF_G.sweep_first && replica - AF_G.sweep_first < AF_G.sweep_rows) {
@@ -1229,6 +1282,10 @@ AF_FN void load_params(State& W, const AfSpikeMark* spikes, const AfOutageMark* 
             case AF_FIELD_SERVER_MAX_IN_SERVICE: tbl_server(W)[col.index].adm_left = v > 0.0 ? (uint32_t)v : 0xFFFFFFFFu; break;
             case AF_FIELD_SERVER_DEADLINE: tbl_deadline(W)[col.index] = v > 0.0 ? v : INF_DEADLINE; break;
             case AF_FIELD_CLIENT_TIMEOUT: W.timeout = v > 0.0 ? v : INF_DEADLINE; break;
+            case AF_FIELD_SERVER_RATE: tbl_rate(W)[col.index].tau = v; break;       // (rate and burst until rl_finish)
+            case AF_FIELD_SERVER_BURST: tbl_rate(W)[col.index].lim = v; break;
+            case AF_FIELD_LB_RATE: W.lb_rl.tau = v; break;
+            case AF_FIELD_LB_BURST: W.lb_rl.lim = v; break;
             default: break;
             }
         }
@@ -1244,6 +1301,11 @@ AF_FN void load_params(State& W, const AfSpikeMark* spikes, const AfOutageMark* 
             w_sync();
         }
     }
+    // rate limits (DESIGN.md §3.14): each site's (rate, burst) of the scenario or the row -> (tau, L)
+#pragma unroll 1
+    for (int32_t i = lane; i < AF_L.n_servers; i += WARP) rl_finish(tbl_rate(W)[i].tau, tbl_rate(W)[i].lim);
+    if (lane == 0) rl_finish(W.lb_rl.tau, W.lb_rl.lim);
+    w_sync();
     if (AF_G.redo_list) {                            // a re-run: the first pass left partial counts in the accumulating outputs
         if (AF_L.collect_hist) for (int32_t b = lane; b < AF_HIST_BINS; b += WARP) AF_G.hist[W.local * AF_HIST_BINS + (uint32_t)b] = 0;
         if (AF_L.collect_thr) for (int32_t b = lane; b < AF_L.horizon_s; b += WARP) AF_G.thr[W.local * (uint64_t)AF_L.horizon_s + (uint32_t)b] = 0;
@@ -1321,6 +1383,7 @@ AF_IN void run_replica(State& W, uint64_t local_index, const BandArgs& band, con
     {
         const uint64_t r = id - tl.first;
         const bool own = r < tl.rows;
+        W.lb_rl.tau = band.lb_rate; W.lb_rl.lim = (double)band.lb_burst;
         load_params(W, own ? tl.spikes + r * (uint64_t)AF_L.n_spike : AF_G.spikes, own ? tl.outages + r * (uint64_t)AF_L.n_outage : AF_G.outages,
                     band.client_timeout);
     }
@@ -1401,6 +1464,7 @@ AF_IN void run_replica(State& W, uint64_t local_index, const BandArgs& band, con
         if (lane_id() == 0) band.late[local_index] = W.late;
         w_sync();
     }
+    if (band.throttled != nullptr) rl_write_back(W, band.throttled + local_index * ((uint64_t)AF_L.n_servers + 1));
 }
 AF_IN void run_replica(State& W, uint64_t local_index, const BandArgs& band, const TimelineArgs& tl) {
     const StreamArgs none = {};

@@ -435,6 +435,10 @@ struct af_engine {
     // §3.13); written by launches with a deadline or a timeout somewhere, which also upload the lane's dl_base table
     DevBuf d_expired, d_late, d_l_dl;
     bool last_dl = false;
+    // requests each site throttled at its rate limit, [n][n_servers + 1] (DESIGN.md §3.14); written by launches with a
+    // rate limit somewhere, which also upload the lane's rl_base table
+    DevBuf d_throttled, d_l_rl;
+    bool last_rl = false;
     bool last_occ = false; int32_t last_occ_bits = 0, last_occ_cols = 0;
 
     int fail(int code, const std::string& m) { err = m; return code; }
@@ -520,7 +524,7 @@ void af_engine_destroy(af_engine* e) {
                       &e->d_okey, &e->d_oidx, &e->d_order, &e->d_okey64, &e->d_sort_tmp,
                       &e->d_band_group, &e->d_band, &e->d_band_from, &e->d_lat, &e->d_lat_from,
                       &e->d_dist_slot, &e->d_dist, &e->d_occ, &e->d_tl_spikes, &e->d_tl_l_spikes, &e->d_tl_outages, &e->d_streams,
-                      &e->d_expired, &e->d_late, &e->d_l_dl};
+                      &e->d_expired, &e->d_late, &e->d_l_dl, &e->d_throttled, &e->d_l_rl};
     for (DevBuf* b : bufs) b->release();
     cudaEventDestroy(e->ev_begin); cudaEventDestroy(e->ev_sim); cudaEventDestroy(e->ev_end);
     cudaStreamDestroy(e->stream);
@@ -596,7 +600,14 @@ int af_sweep_upload(af_engine* e, const AfSweep* sw, uint64_t first_replica) {
         case AF_FIELD_LB_ALGORITHM: lim = 1; break;
         case AF_FIELD_SERVER_DEADLINE: lim = s.n_servers; break;
         case AF_FIELD_CLIENT_TIMEOUT: lim = 1; break;
+        case AF_FIELD_SERVER_RATE: case AF_FIELD_SERVER_BURST: lim = s.n_servers; break;
+        case AF_FIELD_LB_RATE: case AF_FIELD_LB_BURST: lim = s.n_lb_edges > 0 ? 1 : 0; break;   // (afh::ratelimit_sweep_fits says why)
         default: return e->fail(AF_ERR_INVALID, "sweep: unknown field id");
+        }
+        if (lim == 0 && (f == AF_FIELD_LB_RATE || f == AF_FIELD_LB_BURST)) {
+            std::string why;
+            afh::ratelimit_sweep_fits(s, sw->columns + c, 1, sw->values, 0, why);
+            return e->fail(AF_ERR_INVALID, why);
         }
         if (i < 0 || i >= lim) return e->fail(AF_ERR_INVALID, "sweep: column index out of range");
     }
@@ -611,6 +622,8 @@ int af_sweep_upload(af_engine* e, const AfSweep* sw, uint64_t first_replica) {
             case AF_FIELD_ENDPOINT_RAM: ok = ok && v >= 0.0 && v <= 2147483647.0; break;
             case AF_FIELD_SERVER_MAX_IN_SERVICE: break;                         // afh::admission_sweep_fits
             case AF_FIELD_SERVER_DEADLINE: case AF_FIELD_CLIENT_TIMEOUT: break;  // afh::deadline_sweep_fits
+            case AF_FIELD_SERVER_RATE: case AF_FIELD_SERVER_BURST:
+            case AF_FIELD_LB_RATE: case AF_FIELD_LB_BURST: break;              // afh::ratelimit_sweep_fits
             case AF_FIELD_EDGE_MEAN: {
                 const int d = s.edges[sw->columns[c].index].dist;
                 ok = ok && (v >= 0.0 || d == AF_DIST_LOG_NORMAL || d == AF_DIST_NORMAL);
@@ -636,7 +649,8 @@ int af_sweep_upload(af_engine* e, const AfSweep* sw, uint64_t first_replica) {
         std::string why;
         if (!afh::lb_sweep_fits(s, sw->columns, sw->n_columns, sw->values, sw->n_rows, why)
             || !afh::admission_sweep_fits(sw->columns, sw->n_columns, sw->values, sw->n_rows, why)
-            || !afh::deadline_sweep_fits(sw->columns, sw->n_columns, sw->values, sw->n_rows, why)) return e->fail(AF_ERR_INVALID, why);
+            || !afh::deadline_sweep_fits(sw->columns, sw->n_columns, sw->values, sw->n_rows, why)
+            || !afh::ratelimit_sweep_fits(s, sw->columns, sw->n_columns, sw->values, sw->n_rows, why)) return e->fail(AF_ERR_INVALID, why);
     }
     e->h_sweep_cols.assign(sw->columns, sw->columns + sw->n_columns);
     e->h_sweep_alias = aflh::column_aliases(sw->values, sw->n_rows, sw->n_columns);
@@ -1026,6 +1040,7 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
         if ((rc = upload_vec(e, e->d_l_lb, e->lt.lb, "lane tables"))) return rc;
         if ((rc = upload_vec(e, e->d_l_cols, e->lt.cols, "lane tables"))) return rc;
         if ((rc = upload_vec(e, e->d_l_dl, e->lt.dl_base, "lane tables"))) return rc;
+        if ((rc = upload_vec(e, e->d_l_rl, e->lt.rl_base, "lane tables"))) return rc;
         AF_CUDA(e, e->d_counter2.ensure(8), "work counter");
         AF_CUDA(e, e->d_redo_list.ensure(n * 4), "flagged-replica list");
         AF_CUDA(e, e->d_redo_count.ensure(4), "flagged-replica count");
@@ -1059,6 +1074,8 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
     const bool adm = afh::admission_launch(e->sc, e->h_sweep_cols.data(), e->sweep_cols);
     if (adm) AF_CUDA(e, e->d_rejected.ensure(n * (uint64_t)L.n_servers * 4), "rejection counts");
     const bool dl = afh::deadline_launch(e->sc, e->h_sweep_cols.data(), e->sweep_cols);
+    const bool rl = afh::ratelimit_launch(e->sc, e->h_sweep_cols.data(), e->sweep_cols);
+    if (rl) AF_CUDA(e, e->d_throttled.ensure(n * ((uint64_t)L.n_servers + 1) * 4), "throttle counts");
     if (dl) {
         AF_CUDA(e, e->d_expired.ensure(n * (uint64_t)L.n_servers * 4), "expiry counts");
         AF_CUDA(e, e->d_late.ensure(n * 4), "late counts");
@@ -1110,6 +1127,8 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
     band.server_expired = dl ? (uint32_t*)e->d_expired.p : nullptr;
     band.late = dl ? (uint32_t*)e->d_late.p : nullptr;
     band.client_timeout = e->sc.client_timeout;
+    band.throttled = rl ? (uint32_t*)e->d_throttled.p : nullptr;
+    band.lb_rate = e->sc.lb_rate_limit; band.lb_burst = e->sc.lb_burst;
     if (occ) { band.occ = (uint64_t*)e->d_occ.p; band.occ_scale = ldexp(1.0, e->occ_opt.frac_bits); }
     afc::TimelineArgs tl = {};
     if (e->tl_rows) {
@@ -1169,6 +1188,8 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
         C.stream_of = rs.stream_of; C.stream_first = rs.first; C.stream_rows = rs.rows;
         C.server_rejected = band.server_rejected;
         C.dl_base = C.dl ? (const double*)e->d_l_dl.p : nullptr;
+        C.rl_base = C.rl ? (const double*)e->d_l_rl.p : nullptr;
+        C.throttled = band.throttled;
         C.server_expired = band.server_expired; C.late = band.late;
     }
 
@@ -1193,6 +1214,7 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
         AF_CUDA(e, cudaMemsetAsync(e->d_expired.p, 0, n * (uint64_t)L.n_servers * 4, e->stream), "memset expiry counts");
         AF_CUDA(e, cudaMemsetAsync(e->d_late.p, 0, n * 4, e->stream), "memset late counts");
     }
+    if (rl) AF_CUDA(e, cudaMemsetAsync(e->d_throttled.p, 0, n * ((uint64_t)L.n_servers + 1) * 4, e->stream), "memset throttle counts");
     {   // the pull order: (work, local index) heaviest first; then the first wave grouped by estimate
         uint32_t* key = (uint32_t*)e->d_okey.p; uint32_t* idx = (uint32_t*)e->d_oidx.p; uint32_t* order = (uint32_t*)e->d_order.p;
         uint64_t* key64 = (uint64_t*)e->d_okey64.p;
@@ -1249,7 +1271,7 @@ int af_run(af_engine* e, uint64_t seed, uint64_t begin, uint64_t end) {
         e->launches += 1;
     }
     AF_CUDA(e, cudaEventRecord(e->ev_end, e->stream), "event");
-    e->last_n = n; e->ran = true; e->timing_valid = false; e->last_adm = adm; e->last_dl = dl;
+    e->last_n = n; e->ran = true; e->timing_valid = false; e->last_adm = adm; e->last_dl = dl; e->last_rl = rl;
     e->last_lane = lane; e->last_warp = warp; e->last_lean = lean; e->last_lane_warps = lane_warps;
     e->last_bands = bands; e->last_band_groups = e->band_groups; e->last_band_ticks = (uint32_t)band_ticks;
     e->last_band_stride = band_stride;
@@ -1366,6 +1388,14 @@ int af_fetch_server_expired(af_engine* e, uint32_t* out, uint64_t n) {
         return AF_OK;
     }
     return fetch(e, out, e->d_expired, n * (uint64_t)e->L.n_servers * 4, n, "expiry counts D2H");
+}
+int af_fetch_throttled(af_engine* e, uint32_t* out, uint64_t n) {
+    const uint64_t bytes = e ? n * ((uint64_t)e->L.n_servers + 1) * 4 : 0;
+    if (e && e->ran && out && n == e->last_n && !e->last_rl) {       // no rate limit anywhere: nothing was throttled
+        memset(out, 0, bytes);
+        return AF_OK;
+    }
+    return fetch(e, out, e->d_throttled, bytes, n, "throttle counts D2H");
 }
 int af_fetch_late(af_engine* e, uint32_t* out, uint64_t n) {
     if (e && e->ran && out && n == e->last_n && !e->last_dl) {       // no timeout anywhere: nothing was late

@@ -62,7 +62,14 @@ inline bool validate(const AfScenario& s, std::string& err) {
                  "server %d: endpoint range", i);
         AF_CHECK(v.max_in_service >= 0, "server %d: max_in_service=%d must be >= 0 (0 = no admission limit)", i, v.max_in_service);
         AF_CHECK(isfinite(v.deadline) && v.deadline >= 0.0, "server %d: deadline=%g must be finite and >= 0 (0 = none)", i, v.deadline);
+        AF_CHECK(isfinite(v.rate_limit) && v.rate_limit >= 0.0, "server %d: rate_limit=%g must be finite and >= 0 (0 = none)",
+                 i, v.rate_limit);
+        AF_CHECK(v.burst >= 0, "server %d: burst=%d must be >= 0 (0 reads as 1)", i, v.burst);
     }
+    AF_CHECK(isfinite(s.lb_rate_limit) && s.lb_rate_limit >= 0.0, "lb_rate_limit=%g must be finite and >= 0 (0 = none)",
+             s.lb_rate_limit);
+    AF_CHECK(s.lb_burst >= 0, "lb_burst=%d must be >= 0 (0 reads as 1)", s.lb_burst);
+    AF_CHECK(s.lb_rate_limit == 0.0 || s.n_lb_edges > 0, "lb_rate_limit=%g: the scenario has no load balancer", s.lb_rate_limit);
     AF_CHECK(isfinite(s.client_timeout) && s.client_timeout >= 0.0, "client_timeout=%g must be finite and >= 0 (0 = none)",
              s.client_timeout);
     for (int i = 0; i < s.n_endpoints; ++i) {
@@ -165,6 +172,47 @@ inline bool deadline_sweep_fits(const AfSweepColumn* cols, int32_t n_cols, const
                 snprintf(b, sizeof b, "sweep: row %llu column %d (%s %d): value %g is not a finite number of seconds >= 0",
                          (unsigned long long)r, c, f == AF_FIELD_SERVER_DEADLINE ? "server_deadline, server" : "client_timeout, index",
                          cols[c].index, v);
+                err = b;
+                return false;
+            }
+        }
+    }
+    return true;
+}
+
+// Does a launch have a rate limit somewhere (DESIGN.md §3.14)?  A scenario rate, or a sweep column over
+// AF_FIELD_SERVER_RATE / AF_FIELD_SERVER_BURST / AF_FIELD_LB_RATE / AF_FIELD_LB_BURST (even one of zeros): only such
+// launches lay out the kernels' token buckets and fill the throttled output.
+inline bool ratelimit_launch(const AfScenario& s, const AfSweepColumn* cols, int32_t n_cols) {
+    if (s.lb_rate_limit > 0.0) return true;
+    for (int32_t i = 0; i < s.n_servers; ++i) if (s.servers[i].rate_limit > 0.0) return true;
+    for (int32_t c = 0; c < n_cols; ++c)
+        if (cols[c].field >= AF_FIELD_SERVER_RATE && cols[c].field <= AF_FIELD_LB_BURST) return true;
+    return false;
+}
+
+// af_sweep_upload's check of the rate-limit columns: a rate finite and >= 0, a burst an integer in [1, 2^31) (naming the
+// row), and no LB column on a scenario without a load balancer.  Index ranges are checked with the other fields'.
+inline bool ratelimit_sweep_fits(const AfScenario& s, const AfSweepColumn* cols, int32_t n_cols, const double* vals,
+                                 uint64_t n_rows, std::string& err) {
+    static const char* const names[] = {"server_rate, server", "server_burst, server", "lb_rate, index", "lb_burst, index"};
+    char b[200];
+    for (int32_t c = 0; c < n_cols; ++c) {
+        const int32_t f = cols[c].field;
+        if (f < AF_FIELD_SERVER_RATE || f > AF_FIELD_LB_BURST) continue;
+        const char* name = names[f - AF_FIELD_SERVER_RATE];
+        if ((f == AF_FIELD_LB_RATE || f == AF_FIELD_LB_BURST) && s.n_lb_edges == 0) {
+            snprintf(b, sizeof b, "sweep: column %d (%s %d): the scenario has no load balancer", c, name, cols[c].index);
+            err = b;
+            return false;
+        }
+        const bool rate = f == AF_FIELD_SERVER_RATE || f == AF_FIELD_LB_RATE;
+        for (uint64_t r = 0; r < n_rows; ++r) {
+            const double v = vals[r * (uint64_t)n_cols + (uint64_t)c];
+            const bool ok = rate ? v >= 0.0 && isfinite(v) : v >= 1.0 && v <= 2147483647.0 && v == floor(v);   // (NaN fails)
+            if (!ok) {
+                snprintf(b, sizeof b, "sweep: row %llu column %d (%s %d): value %g is not %s", (unsigned long long)r, c, name,
+                         cols[c].index, v, rate ? "a finite rate >= 0 (0 = none)" : "an integer burst in [1, 2^31)");
                 err = b;
                 return false;
             }

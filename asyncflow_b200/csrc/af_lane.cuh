@@ -215,6 +215,14 @@ struct Cfg {
     int32_t dl, o64_dl, c_exp, dl_pad;
     const double* dl_base;
     uint32_t* server_expired; uint32_t* late;
+    // rate limits (DESIGN.md §3.14), laid out only when rl != 0 (aflh::Tables.rl).  Site k (server k; k = n_servers: the
+    // load balancer) keeps its theoretical arrival time in the 64-bit word o64_rl + k and its tau and tolerance L in the
+    // 64-bit global-tier elements gi_rl + 2k and gi_rl + 2k + 1 (tau = 0: no limit), computed at the replica's start from
+    // the scenario's rate rl_base[2k] and burst rl_base[2k + 1], then the sweep row.  The cold word c_thr + k counts the
+    // requests it throttled, written to throttled[local * (n_servers + 1) + k] at write-back
+    int32_t rl, o64_rl, gi_rl, c_thr;
+    const double* rl_base;
+    uint32_t* throttled;
 };
 // Cfg.lb_algo of a launch that sweeps the load-balancer algorithm (AF_FIELD_LB_ALGORITHM; DESIGN.md §3.11): each replica
 // reads its own from the 32-bit word right after its LB order, o32_lb + n_lb_edges
@@ -492,6 +500,46 @@ AFL_COLD void dl_write_back(const Mem m, uint64_t local) {
     for (int32_t i = 0; i < AFL_C.n_servers; ++i)
         AFL_C.server_expired[local * (uint64_t)AFL_C.n_servers + (uint32_t)i] = c32_ld(m, AFL_C.c_exp + i);
     AFL_C.late[local] = c32_ld(m, AFL_C.c_exp + AFL_C.n_servers);
+}
+
+// Rate limits (Cfg.rl; DESIGN.md §3.14; the full build only -- aflh::lean_launch).  Site k's process takes a request at
+// `now`: true when its bucket throttles it (counted; the caller releases the record, as for a shed request), else the
+// request spends a token.  The check itself is afr::rl_pass, shared with the warp engine.
+AFL_COLD bool rl_throttle(const Mem m, double now, int32_t k) {
+    const double tau = afr::u2d(*g64p(m, AFL_C.gi_rl + 2 * k));
+    if (tau == 0.0) return false;
+    double tat = f64_ld(m, AFL_C.o64_rl + k);
+    if (afr::rl_pass(tat, now, tau, afr::u2d(*g64p(m, AFL_C.gi_rl + 2 * k + 1)))) {
+        f64_st(m, AFL_C.o64_rl + k, tat);
+        return false;
+    }
+    c32_st(m, AFL_C.c_thr + k, c32_ld(m, AFL_C.c_thr + k) + 1u);
+    return true;
+}
+// start_replica: every site's rate and burst from the scenario (a sweep row overrides them after; rl_finish turns them
+// into tau and L), a full bucket, nothing throttled yet
+AFL_COLD void rl_start(const Mem m) {
+    for (int32_t k = 0; k <= AFL_C.n_servers; ++k) {
+        *g64p(m, AFL_C.gi_rl + 2 * k) = afr::d2u(AFL_C.rl_base[2 * k]);
+        *g64p(m, AFL_C.gi_rl + 2 * k + 1) = afr::d2u(AFL_C.rl_base[2 * k + 1]);
+        f64_st(m, AFL_C.o64_rl + k, 0.0);
+        c32_st(m, AFL_C.c_thr + k, 0);
+    }
+}
+// ... after the sweep row: (rate, burst) -> (tau, L); a rate of 0 is no limit (tau = 0), a burst below 1 reads as 1
+AFL_COLD void rl_finish(const Mem m) {
+    for (int32_t k = 0; k <= AFL_C.n_servers; ++k) {
+        const double rate = afr::u2d(*g64p(m, AFL_C.gi_rl + 2 * k)), burst = afr::u2d(*g64p(m, AFL_C.gi_rl + 2 * k + 1));
+        double tau = 0.0, lim = 0.0;
+        if (rate > 0.0) afr::rl_params(rate, burst < 1.0 ? 1.0 : burst, tau, lim);
+        *g64p(m, AFL_C.gi_rl + 2 * k) = afr::d2u(tau);
+        *g64p(m, AFL_C.gi_rl + 2 * k + 1) = afr::d2u(lim);
+    }
+}
+// write_back: the throttled requests of every site of the replica in output slot `local`
+AFL_COLD void rl_write_back(const Mem m, uint64_t local) {
+    for (int32_t k = 0; k <= AFL_C.n_servers; ++k)
+        AFL_C.throttled[local * (uint64_t)(AFL_C.n_servers + 1) + (uint32_t)k] = c32_ld(m, AFL_C.c_thr + k);
 }
 
 // start_replica: every server's word from the scenario (a sweep row overrides it after), no rejection yet
@@ -1021,6 +1069,7 @@ AFL_IN void start_replica(St& W, const Mem& m, uint64_t local_index) {
     }
     if (!kLean && C.adm) adm_start(m);
     if (!kLean && C.dl) dl_start(m);
+    if (!kLean && C.rl) rl_start(m);
 #pragma unroll 1
     for (int32_t i = 0; i < C.n_servers + 2; ++i) {
         c32_st(m, ib_word((uint32_t)i, IB_HEAD), NIL); c32_st(m, ib_word((uint32_t)i, IB_TAIL), NIL); c32_st(m, ib_word((uint32_t)i, IB_PENDING), 1);
@@ -1047,6 +1096,11 @@ AFL_IN void start_replica(St& W, const Mem& m, uint64_t local_index) {
                 f64_st(m, C.o64_dl + (col.field == AF_FIELD_SERVER_DEADLINE ? col.index : C.n_servers), v > 0.0 ? v : afr::u2d(INF_BITS));
                 continue;
             }
+            if (col.field >= AF_FIELD_SERVER_RATE && col.field <= AF_FIELD_LB_BURST) {   // rate / burst of a server or the LB
+                const int32_t k = col.field <= AF_FIELD_SERVER_BURST ? col.index : C.n_servers;
+                *g64p(m, C.gi_rl + 2 * k + ((col.field - AF_FIELD_SERVER_RATE) & 1)) = afr::d2u(v);
+                continue;
+            }
         }
         switch (col.field) {
         case AF_FIELD_SERVER_CPU_CORES: i32_st(m, sv_word((uint32_t)col.index, SV_CPU_FREE), (int32_t)v); break;
@@ -1056,6 +1110,7 @@ AFL_IN void start_replica(St& W, const Mem& m, uint64_t local_index) {
         default: break;
         }
     }
+    if (!kLean && C.rl) rl_finish(m);
     if (uncovered) {                                  // the LB order without the edges the row uncovers
         int32_t n = 0;
 #pragma unroll 1
@@ -1096,6 +1151,7 @@ AFL_IN void write_back(St& W, const Mem& m) {
     }
     if (!kLean && C.adm) adm_write_back(m, local);
     if (!kLean && C.dl) dl_write_back(m, local);
+    if (!kLean && C.rl) rl_write_back(m, local);
     AfReplicaStats st;
     st.n_events = W.n_events; st.generated = W.generated; st.completed = W.completed;
     st.flags = W.flags; st.n_ticks = W.n_ticks; st.peak_events = W.peak_ev; st.peak_requests = W.peak_rq;
@@ -1355,7 +1411,8 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                 if (from_box) consumer_get(W, m, node);        // the dispatcher loops back to get() first (fused: the box is empty and
                                                                // the consumer already marked as waiting -- nothing to do)
                 const ServerP sp = ro(C.servers + sidx);
-                const bool shed = !kLean && C.adm && adm_shed(m, sidx, sp.out_edge);
+                bool shed = false;                             // throttled at its rate limit (§3.14), then shed at its cap
+                if constexpr (!kLean) shed = (C.rl && rl_throttle(m, W.now, (int32_t)sidx)) || (C.adm && adm_shed(m, sidx, sp.out_edge));
                 if (shed) rq_release(W, m, slot);             // shed at the door: the request is gone
                 else {
                     pack += 1;                                     // record_hop(SERVER)
@@ -1400,9 +1457,12 @@ AFL_IN void run_lane(const Mem& m, NextFn next_index, ConvFn converge) {
                     }
                 } else {
                     const int32_t lb = C.o32_lb, n = W.lb_n;
+                    bool throttled = false;                    // throttled at the LB's rate limit: gone before the pick (§3.14)
+                    if constexpr (!kLean) throttled = C.rl && rl_throttle(m, W.now, C.n_servers);
+                    if (throttled) { rq_release(W, m, slot); if (from_box) consumer_get(W, m, NODE_LB); }
                     // every covered server is down: the reference dies here (StopIteration inside round_robin);
                     // the replica stops and says so (flatten() rejects timelines that can reach this state)
-                    if (AFL_UNLIKELY(n <= 0)) { rq_pack_set(W, m, slot, pack); W.flags |= AF_FLAG_LB_EMPTY; }
+                    else if (AFL_UNLIKELY(n <= 0)) { rq_pack_set(W, m, slot, pack); W.flags |= AF_FLAG_LB_EMPTY; }
                     else {
                         uint32_t pick = w32_ld(m, lb);
                         // (a launch that sweeps the algorithm keeps each replica's next to its LB order)

@@ -20,6 +20,10 @@ struct Tables {
     // dl_base (the scenario's deadline of each server, then its client timeout; 0: none)
     int32_t dl = 0;
     std::vector<double> dl_base;
+    // 1: a rate limit somewhere (afh::ratelimit_launch): n_servers + 1 64-bit words per lane (each site's tat) and
+    // 2 (n_servers + 1) in its global tier (tau, L), from rl_base (each server's rate and burst, then the LB's)
+    int32_t rl = 0;
+    std::vector<double> rl_base;
 };
 
 // Scenario (+ the sweep's columns) -> the kernel's read-only tables.  A column over a field the kernel
@@ -42,8 +46,10 @@ inline bool build_tables(const AfScenario& s, const AfSweepColumn* cols, int32_t
         v.ep_begin = (uint32_t)a.endpoint_begin; v.n_ep = (uint32_t)a.n_endpoints; v.c_cores = v.c_ram = -1; v.max_in_service = a.max_in_service;
         if (a.max_in_service > 0) t.adm = 1;
         if (a.deadline > 0.0) t.dl = 1;
+        if (a.rate_limit > 0.0) t.rl = 1;
     }
     if (s.client_timeout > 0.0) t.dl = 1;
+    if (s.lb_rate_limit > 0.0) t.rl = 1;
     t.endpoints.resize((size_t)s.n_endpoints);
     for (int i = 0; i < s.n_endpoints; ++i) {
         const AfEndpoint& a = s.endpoints[i]; afl::EndpointP& p = t.endpoints[(size_t)i];
@@ -87,6 +93,10 @@ inline bool build_tables(const AfScenario& s, const AfSweepColumn* cols, int32_t
         case AF_FIELD_SERVER_MAX_IN_SERVICE: k.base = s.servers[i].max_in_service; t.adm = 1; break;
         case AF_FIELD_SERVER_DEADLINE: k.base = s.servers[i].deadline; t.dl = 1; break;
         case AF_FIELD_CLIENT_TIMEOUT: k.base = s.client_timeout; t.dl = 1; break;
+        case AF_FIELD_SERVER_RATE: k.base = s.servers[i].rate_limit; t.rl = 1; break;
+        case AF_FIELD_SERVER_BURST: k.base = s.servers[i].burst; t.rl = 1; break;
+        case AF_FIELD_LB_RATE: k.base = s.lb_rate_limit; t.rl = 1; break;
+        case AF_FIELD_LB_BURST: k.base = s.lb_burst; t.rl = 1; break;
         default: err = "sweep: unknown field id"; return false;
         }
 #undef AFLH_SLOT
@@ -97,6 +107,11 @@ inline bool build_tables(const AfScenario& s, const AfSweepColumn* cols, int32_t
         t.dl_base.resize((size_t)s.n_servers + 1);
         for (int i = 0; i < s.n_servers; ++i) t.dl_base[(size_t)i] = s.servers[i].deadline;
         t.dl_base[(size_t)s.n_servers] = s.client_timeout;
+    }
+    if (t.rl) {
+        t.rl_base.resize(2 * ((size_t)s.n_servers + 1));
+        for (int i = 0; i < s.n_servers; ++i) { t.rl_base[2 * (size_t)i] = s.servers[i].rate_limit; t.rl_base[2 * (size_t)i + 1] = s.servers[i].burst; }
+        t.rl_base[2 * (size_t)s.n_servers] = s.lb_rate_limit; t.rl_base[2 * (size_t)s.n_servers + 1] = s.lb_burst;
     }
     return true;
 }
@@ -211,7 +226,7 @@ constexpr int32_t LANE_REQUEST_CAPACITY = 2048;
 // LB order, the gauges' dirty bits (32-bit).  (The gauges' sums / maxima and the send counters are write-only: global tier.)
 inline int32_t fixed_lane_bytes(const AfScenario& s, const Tables& t) {
     const int32_t n_series = 3 * s.n_servers + s.n_edges;
-    const int32_t fix64 = (s.n_spike_marks > 0 ? s.n_edges : 0) + t.n_row + t.dl * (s.n_servers + 1);
+    const int32_t fix64 = (s.n_spike_marks > 0 ? s.n_edges : 0) + t.n_row + t.dl * (s.n_servers + 1) + t.rl * (s.n_servers + 1);
     const int32_t fix32 = s.n_edges + afl::SV_WORDS * s.n_servers + s.n_lb_edges + t.lb_algo_word + t.adm * s.n_servers + (n_series + 31) / 32;
     return 8 * fix64 + 4 * fix32;
 }
@@ -229,7 +244,8 @@ inline void pool_split(const afl::Cfg& C, int32_t need, int32_t& ev_s, int32_t& 
 // every edge normal or exponential, every server with one endpoint, no admission limit (a scenario limit or an
 // AF_FIELD_SERVER_MAX_IN_SERVICE column in `cols`: the lean loop leaves the check out, and the loop `bench.py` runs keeps
 // the instructions it had), and no deadline or client timeout (likewise; AF_FIELD_SERVER_DEADLINE /
-// AF_FIELD_CLIENT_TIMEOUT).  No other sweep column can change any of these.
+// AF_FIELD_CLIENT_TIMEOUT), and no rate limit (likewise; a scenario rate, or a column over any of the four rate-limit
+// fields).  No other sweep column can change any of these.
 inline bool lean_launch(const AfScenario& s, int32_t trace_replicas, const AfSweepColumn* cols = nullptr, int32_t n_cols = 0) {
     if (s.n_spike_marks > 0 || s.n_outage_marks > 0 || trace_replicas > 0) return false;
     for (int i = 0; i < s.n_servers; ++i)
@@ -237,9 +253,13 @@ inline bool lean_launch(const AfScenario& s, int32_t trace_replicas, const AfSwe
     if (s.client_timeout > 0.0) return false;
     for (int i = 0; i < s.n_servers; ++i)
         if (s.servers[i].deadline > 0.0) return false;
+    if (s.lb_rate_limit > 0.0) return false;
+    for (int i = 0; i < s.n_servers; ++i)
+        if (s.servers[i].rate_limit > 0.0) return false;
     for (int32_t c = 0; c < n_cols; ++c)
         if (cols[c].field == AF_FIELD_SERVER_MAX_IN_SERVICE || cols[c].field == AF_FIELD_SERVER_DEADLINE
-            || cols[c].field == AF_FIELD_CLIENT_TIMEOUT) return false;
+            || cols[c].field == AF_FIELD_CLIENT_TIMEOUT
+            || (cols[c].field >= AF_FIELD_SERVER_RATE && cols[c].field <= AF_FIELD_LB_BURST)) return false;
     for (int i = 0; i < s.n_edges; ++i)
         if (s.edges[i].dist != AF_DIST_NORMAL && s.edges[i].dist != AF_DIST_EXPONENTIAL) return false;
     for (int i = 0; i < s.n_servers; ++i)
@@ -270,7 +290,7 @@ inline bool make_cfg(const AfScenario& s, const AfOptions& o, const Tables& t, i
     int32_t rq_total = o.request_capacity > 0 ? o.request_capacity : LANE_REQUEST_CAPACITY;
     if (rq_total > (int32_t)afl::SLOT_MASK) rq_total = (int32_t)afl::SLOT_MASK;
     // fixed part of a lane's shared memory
-    const int32_t fix64 = (C.n_spike > 0 ? C.n_edges : 0) + C.n_row + t.dl * (C.n_servers + 1);
+    const int32_t fix64 = (C.n_spike > 0 ? C.n_edges : 0) + C.n_row + t.dl * (C.n_servers + 1) + t.rl * (C.n_servers + 1);
     C.n_dirty = (C.n_series + 31) / 32;
     const int32_t fix32 = C.n_edges + afl::SV_WORDS * C.n_servers + C.n_lb_edges + t.lb_algo_word + t.adm * C.n_servers + C.n_dirty;
     int32_t nq_s = 0;                                // zero-delay items: ties only -- the ring starts in the global tier
@@ -299,6 +319,8 @@ inline bool make_cfg(const AfScenario& s, const AfOptions& o, const Tables& t, i
     C.o64_row = e; e += C.n_row;
     C.dl = t.dl; C.o64_dl = e; e += t.dl * (C.n_servers + 1);
     C.dl_base = t.dl ? t.dl_base.data() : nullptr;   // the host copy (the twin runs on it); af_run points at the device's
+    C.rl = t.rl; C.o64_rl = e; e += t.rl * (C.n_servers + 1);
+    C.rl_base = t.rl ? t.rl_base.data() : nullptr;   // (likewise)
     C.n64 = e;
     int32_t w = 0;
     C.o32_conn = w; w += C.n_edges;
@@ -316,12 +338,14 @@ inline bool make_cfg(const AfScenario& s, const AfOptions& o, const Tables& t, i
     C.gi_nq = 0 - nq_s;
     C.gi_acc = afl::NQ_TOTAL - nq_s;
     C.gn64 = C.gi_acc + C.n_series;
+    C.gi_rl = C.gn64; C.gn64 += t.rl * 2 * (C.n_servers + 1);   // each site's tau and L (read at a check only)
     int32_t hcount = rq_total;                       // the `next` link of every record slot
     C.g32_cold = hcount;
     C.c_srvq = 0; C.c_inbox = C.c_srvq + afl::SQ_WORDS * C.n_servers; C.c_drop = C.c_inbox + afl::IB_WORDS * (C.n_servers + 2);
     C.c_rej = C.c_drop + C.n_edges;
     C.c_exp = C.c_rej + t.adm * C.n_servers;
-    hcount += C.c_exp + t.dl * (C.n_servers + 1);
+    C.c_thr = C.c_exp + t.dl * (C.n_servers + 1);
+    hcount += C.c_thr + t.rl * (C.n_servers + 1);
     C.gi_smax = hcount; hcount += C.n_series;
     C.gi_sent = hcount; hcount += C.n_edges;
     C.gn32 = hcount;

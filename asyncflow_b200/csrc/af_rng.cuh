@@ -91,6 +91,32 @@ AF_HD double af_div(double a, double b) {
 #endif
 }
 
+// Rate limits (DESIGN.md §3.14): a site's GCRA token bucket.  A rate r > 0 per second and a burst b >= 1 give
+// tau = 1/r and the tolerance L = (b - 1) * tau, each correctly rounded; the site's state is its theoretical arrival
+// time `tat`.  rl_pass: may a request taken at `now` pass?  (tat - now > L: throttled, tat unchanged; else it spends a
+// token: tat = max(tat, now) + tau.)  The exact f64 operations of tests/des_ratelimit.py, in its order, no contraction.
+AF_HD double af_mul(double a, double b) {
+#if defined(__CUDA_ARCH__)
+    return __dmul_rn(a, b);
+#else
+    return a * b;
+#endif
+}
+AF_HD void rl_params(double rate, double burst, double& tau, double& lim) {
+    tau = af_div(1.0, rate);
+    lim = af_mul(burst - 1.0, tau);
+}
+AF_HD bool rl_pass(double& tat, double now, double tau, double lim) {
+#if defined(__CUDA_ARCH__)
+    if (__dsub_rn(tat, now) > lim) return false;
+    tat = __dadd_rn(tat > now ? tat : now, tau);
+#else
+    if (tat - now > lim) return false;
+    tat = (tat > now ? tat : now) + tau;
+#endif
+    return true;
+}
+
 // The latency histogram's bin of `lat` (AF_HIST_BINS log-linear bins, clamped at both ends): the per-replica
 // histograms and the per-window latency bands bin alike.
 AF_HD int32_t hist_bin(double lat) {

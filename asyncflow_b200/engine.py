@@ -172,6 +172,13 @@ class Engine:
         self._check(self._lib.af_fetch_late(self._h, out.ctypes.data, self._n), "af_fetch_late")
         return out
 
+    def throttled(self, out: np.ndarray | None = None) -> np.ndarray:
+        """Requests each site throttled at its rate limit, ``[n, n_servers + 1]`` (column ``n_servers``: the load
+        balancer) -- ``af_fetch_throttled``."""
+        out = np.empty((self._n, self.flat.n_servers + 1), dtype=np.uint32) if out is None else out
+        self._check(self._lib.af_fetch_throttled(self._h, out.ctypes.data, self._n), "af_fetch_throttled")
+        return out
+
     def histograms(self) -> np.ndarray:
         out = np.empty((self._n, K.AF_HIST_BINS), dtype=np.uint32)
         self._check(self._lib.af_fetch_histograms(self._h, out.ctypes.data, self._n), "af_fetch_histograms")

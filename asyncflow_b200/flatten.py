@@ -132,6 +132,50 @@ def set_deadlines(flat: "FlatScenario", deadlines: dict[str, float] | None, *, c
         flat.pod.client_timeout = t
 
 
+def _rate(x: Any) -> float:
+    """A rate limit in requests per second as a float, NaN unless it is finite and >= 0 (bools refused)."""
+    return _seconds(x)
+
+
+def _burst(x: Any, lo: int = 1) -> float:
+    """A burst as a float, NaN unless it is an integer in [lo, 2**31) (bools refused)."""
+    v = _limit(x)
+    return v if v >= lo else np.nan
+
+
+def set_rate_limits(flat: "FlatScenario", limits: dict[str, tuple[float, int]] | None, *,
+                    lb: tuple[float, int] | None = None) -> None:
+    """The scenario's rate limits (DESIGN.md §3.14): ``limits[server_id] = (rate, burst)`` (servers left out keep
+    theirs) and the load balancer's ``lb = (rate, burst)`` (``None``: kept), a rate in requests per second (0 = none)
+    and a burst, an integer >= 0 (0 reads as 1).  ``KeyError`` for an unknown server, ``ValueError`` for a bad value or
+    an LB limit on a scenario without a load balancer."""
+    def pair(what: str, v: Any) -> tuple[float, int]:
+        try:
+            r, b = v
+        except (TypeError, ValueError):
+            msg = f"{what}: {v!r} is not a (rate, burst) pair"
+            raise ValueError(msg) from None
+        rr, bb = _rate(r), _burst(b, lo=0)
+        if rr != rr:
+            msg = f"{what}: rate {r!r} is not a finite number of requests per second >= 0"
+            raise ValueError(msg)
+        if bb != bb:
+            msg = f"{what}: burst {b!r} is not an integer in [0, 2**31)"
+            raise ValueError(msg)
+        return rr, int(bb)
+    for sid, v in (limits or {}).items():
+        if sid not in flat.server_ids:
+            msg = f"rate limits: no server {sid!r} (servers: {list(flat.server_ids)})"
+            raise KeyError(msg)
+        srv = flat.pod.servers[flat.server_ids.index(sid)]
+        srv.rate_limit, srv.burst = pair(f"rate limits: server {sid!r}", v)
+    if lb is not None:
+        if flat.lb_id is None:
+            msg = "rate limits: the scenario has no load balancer to limit"
+            raise ValueError(msg)
+        flat.pod.lb_rate_limit, flat.pod.lb_burst = pair("rate limits: load balancer", lb)
+
+
 def _rv(d: dict) -> tuple[str, float, float]:
     dist = _s(d.get("distribution") or "poisson")
     var = d.get("variance")
@@ -474,7 +518,9 @@ class SweepSpec:
     ``("lb_covered", server_id)`` (1: behind the load balancer as in the scenario, 0: not; bools accepted) and
     ``("lb_algorithm",)`` (``"round_robin"`` or ``"least_connection"``, enum members or ``K.LB_*`` codes accepted) and
     ``("server_max_in_service", server_id)`` (the server's admission limit, an integer >= 0, 0 = none; DESIGN.md §3.12),
-    ``("server_deadline", server_id)`` and ``("client_timeout",)`` (seconds >= 0, 0 = none; DESIGN.md §3.13).
+    ``("server_deadline", server_id)`` and ``("client_timeout",)`` (seconds >= 0, 0 = none; DESIGN.md §3.13),
+    ``("server_rate"|"server_burst", server_id)`` and ``("lb_rate",)`` / ``("lb_burst",)`` (a rate limit in requests per
+    second, finite and >= 0, 0 = none, and its burst, an integer in [1, 2**31); DESIGN.md §3.14).
 
     A row that uncovers a server simulates the scenario without the load balancer's edge to it (:meth:`payload_for`):
     its round-robin order is the scenario's with that edge left out, and an outage of that server is a no-op.  The
@@ -500,9 +546,14 @@ class SweepSpec:
         arrays = [self._lb_values(flat, sel, v) if sel[0] in ("lb_covered", "lb_algorithm")
                   else self._limits(flat, sel, v) if sel[0] in K.ADMISSION_FIELDS
                   else self._seconds(flat, sel, v) if sel[0] in K.DEADLINE_FIELDS
+                  else self._rates(flat, sel, v) if sel[0] in K.RATE_FIELDS
                   else np.ascontiguousarray(np.broadcast_to(np.asarray(v, dtype=np.float64), (self.n_replicas,)))
                   for sel, v in zip(keys, columns.values())]
         self.covered = self._covered(flat, keys, arrays)
+        # the scenario's rate limits (set_rate_limits), which a row's rate or burst column overrides
+        self._rl_base = ({sid: (float(flat.pod.servers[i].rate_limit), int(flat.pod.servers[i].burst))
+                          for i, sid in enumerate(flat.server_ids)},
+                         (float(flat.pod.lb_rate_limit), int(flat.pod.lb_burst)) if flat.lb_id is not None else None)
         # rows need their own timelines when event times are swept or when a row drops a server that has outage marks
         times = any(k[0] in ("event_start", "event_end") for k in keys) or (
             self.covered is not None and any((~self.covered[:, flat.lb_edges.index(e.target)]).any()
@@ -516,7 +567,7 @@ class SweepSpec:
                     raise KeyError(msg)
                 self.selectors.append((sel, arr))       # carried by the rows' timelines, not by a column
                 continue
-            if name in ("users_mean", "users_sigma", "rate_per_user", "client_timeout"):
+            if name in ("users_mean", "users_sigma", "rate_per_user", "client_timeout", "lb_rate", "lb_burst"):
                 targets = [0]
             elif name.startswith("edge_"):
                 targets = [flat.edge_ids.index(sel[1])]
@@ -540,7 +591,7 @@ class SweepSpec:
                 raise KeyError(msg)
             self.selectors.append((sel, arr))
             for t in targets:
-                cols.append(({**K.FIELDS, **K.LB_FIELDS, **K.ADMISSION_FIELDS, **K.DEADLINE_FIELDS}[name], t))
+                cols.append(({**K.FIELDS, **K.LB_FIELDS, **K.ADMISSION_FIELDS, **K.DEADLINE_FIELDS, **K.RATE_FIELDS}[name], t))
                 vals.append(arr)
         self.n_columns = len(cols)
         self.values = (np.ascontiguousarray(np.stack(vals, axis=1)) if vals
@@ -615,6 +666,59 @@ class SweepSpec:
             raise ValueError(msg)
         return out
 
+    def _rates(self, flat: FlatScenario, sel: tuple, v: Any) -> np.ndarray:
+        """A rate-limit column: a rate finite and >= 0, or a burst, an integer in [1, 2**31) (``KeyError`` /
+        ``ValueError`` naming the row)."""
+        if sel[0] in ("server_rate", "server_burst") and (len(sel) != 2 or sel[1] not in flat.server_ids):
+            msg = f"sweep column {sel!r}: no server {sel[1] if len(sel) > 1 else None!r} (servers: {list(flat.server_ids)})"
+            raise KeyError(msg)
+        if sel[0] in ("lb_rate", "lb_burst"):
+            if flat.lb_id is None:
+                msg = f"sweep column {sel!r}: the scenario has no load balancer to limit"
+                raise ValueError(msg)
+            if len(sel) != 1:
+                msg = f"sweep column {sel!r}: the load balancer's limit takes no index (({sel[0]!r},))"
+                raise KeyError(msg)
+        raw = np.broadcast_to(np.asarray(v, dtype=object), (self.n_replicas,))
+        rate = sel[0].endswith("_rate")
+        out = np.array([_rate(x) if rate else _burst(x) for x in raw], dtype=np.float64)
+        bad = np.isnan(out)
+        if bad.any():
+            r = int(np.flatnonzero(bad)[0])
+            what = ("a rate limit is a finite number of requests per second >= 0 (0: none)" if rate
+                    else "a burst is an integer in [1, 2**31)")
+            msg = f"sweep row {r}: {sel!r} = {raw[r]!r}: {what}"
+            raise ValueError(msg)
+        return out
+
+    def rate_limits_for(self, replica: int) -> tuple[dict[str, tuple[float, int]], tuple[float, int] | None]:
+        """Row ``replica``'s rate limits: ``{server_id: (rate, burst)}`` for every server with a scenario limit or a
+        column, and the load balancer's ``(rate, burst)`` (``None`` without either), from the scenario's limits and this
+        spec's columns (zeros included; a burst of 0 reads as 1)."""
+        base, lb_base = self._rl_base
+        srv = {sid: list(rb) for sid, rb in base.items() if rb[0] > 0.0}
+        lb = list(lb_base) if lb_base is not None and lb_base[0] > 0.0 else None
+        for sel, arr in self.selectors:
+            if sel[0] not in K.RATE_FIELDS:
+                continue
+            k = 0 if sel[0].endswith("_rate") else 1
+            if sel[0].startswith("server_"):
+                srv.setdefault(sel[1], list(base[sel[1]]))[k] = float(arr[replica])
+            else:
+                if lb is None:
+                    lb = list(lb_base)
+                lb[k] = float(arr[replica])
+        pair = lambda rb: (float(rb[0]), max(1, int(rb[1])))  # noqa: E731
+        return {sid: pair(rb) for sid, rb in srv.items()}, (pair(lb) if lb is not None else None)
+
+    def _refuse_rates(self, replica: int, what: str) -> None:
+        srv, lb = self.rate_limits_for(replica)
+        set_ = {**{sid: rb for sid, rb in srv.items() if rb[0] > 0.0}, **({"load_balancer": lb} if lb and lb[0] > 0.0 else {})}
+        if set_:
+            msg = (f"sweep row {replica} sets rate limits {set_}, which {what} cannot express; "
+                   "payload_and_overload() returns the payload with the rate limits, the deadlines and the limits")
+            raise ValueError(msg)
+
     def deadlines_for(self, replica: int) -> tuple[dict[str, float], float | None]:
         """Row ``replica``'s deadlines ``{server_id: seconds}`` and client timeout (``None`` without such a column) from
         this spec's columns (zeros included)."""
@@ -633,10 +737,21 @@ class SweepSpec:
     def payload_and_overload(self, payload: Any, replica: int) -> tuple[dict, dict]:
         """Row ``replica`` as the oracle takes it: the row's payload (:meth:`payload_for` without the overload columns)
         and ``{"admission": {server_id: limit}, "deadline": {server_id: seconds}, "client_timeout": seconds | None}``
-        (0: none; ``None``: the scenario's).  The reference can express none of them."""
+        (0: none; ``None``: the scenario's).  When the sweep has a rate limit (a column, or the scenario's), also
+        ``"rate_limit": {server_id: (rate, burst)}`` and ``"lb_rate_limit": (rate, burst) | None``
+        (:meth:`rate_limits_for`).  The reference can express none of them."""
         dl, to = self.deadlines_for(replica)
-        return self._payload(payload, replica), {"admission": self.admission_for(replica), "deadline": dl,
-                                                 "client_timeout": to}
+        ov = {"admission": self.admission_for(replica), "deadline": dl, "client_timeout": to}
+        if self.has_rate_limits:
+            ov["rate_limit"], ov["lb_rate_limit"] = self.rate_limits_for(replica)
+        return self._payload(payload, replica), ov
+
+    @property
+    def has_rate_limits(self) -> bool:
+        """Does the sweep have a rate limit somewhere: a rate-limit column (zeros included) or a scenario rate?"""
+        base, lb = self._rl_base
+        return (any(sel[0] in K.RATE_FIELDS for sel, _ in self.selectors) or any(r > 0.0 for r, _ in base.values())
+                or (lb is not None and lb[0] > 0.0))
 
     def admission_for(self, replica: int) -> dict[str, int]:
         """Row ``replica``'s admission limits ``{server_id: limit}`` from this spec's columns (zeros included)."""
@@ -648,6 +763,7 @@ class SweepSpec:
         capped row has no payload of its own.  A row with a deadline or a client timeout is refused (``ValueError``):
         use :meth:`payload_and_overload`."""
         self._refuse_deadlines(replica, "payload_and_admission()")
+        self._refuse_rates(replica, "payload_and_admission()")
         return self._payload(payload, replica), self.admission_for(replica)
 
     def _covered(self, flat: FlatScenario, keys: list[tuple], arrays: list[np.ndarray]) -> np.ndarray | None:
@@ -760,10 +876,11 @@ class SweepSpec:
         ``GpuSimulationRunner``) simulates exactly what row ``replica`` of the sweep simulates;
         it is how a sweep point is handed back to the reference for inspection, and how the parity
         tests build the oracle's input.  ``payload`` is the base scenario the sweep was made from.
-        A row with an admission limit, a deadline or a client timeout has no such payload (the reference has none of
-        them): ``ValueError``; use :meth:`payload_and_overload`.
+        A row with an admission limit, a deadline, a client timeout or a rate limit has no such payload (the reference
+        has none of them): ``ValueError``; use :meth:`payload_and_overload`.
         """
         self._refuse_deadlines(replica, "a payload")
+        self._refuse_rates(replica, "a payload")
         capped = {sid: v for sid, v in self.admission_for(replica).items() if v}
         if capped:
             msg = (f"sweep row {replica} sets admission limits {capped}, which a payload cannot express; "

@@ -173,6 +173,8 @@ class ReplicaResults:
     server_rejected: dict[str, int] = field(default_factory=dict)   # requests each server shed at its admission limit
     server_expired: dict[str, int] = field(default_factory=dict)    # requests each server dropped past its deadline
     late: int = 0                                                    # completions later than the client timeout
+    server_throttled: dict[str, int] = field(default_factory=dict)  # requests each server throttled at its rate limit
+    lb_throttled: int = 0                                            # requests the load balancer throttled
 
     # -- analyzer-compatible getters (metrics/analyzer.py:147-262) -------------
     def list_server_ids(self) -> list[str]:
@@ -306,6 +308,10 @@ class SweepResults:
         # timeout, [n] u32 (zeros without deadlines / a timeout; DESIGN.md §3.13).  Goodput: completed - late
         self.server_expired = np.zeros_like(self.server_rejected)
         self.late = np.zeros(len(stats), dtype=np.uint32)
+        # requests each server throttled at its rate limit, [n, n_servers] u32, and the load balancer throttled, [n] u32
+        # (zeros without rate limits; DESIGN.md §3.14)
+        self.server_throttled = np.zeros_like(self.server_rejected)
+        self.lb_throttled = np.zeros(len(stats), dtype=np.uint32)
         self.rows: np.ndarray | None = None      # sweep row of each result row (set by SweepRunner)
         self.streams: np.ndarray | None = None   # random stream of each result row (SweepRunner.stream_ids; set by collect)
         self.traced: list[ReplicaResults] = []    # full clocks + sampled series of the first `trace_replicas` replica ids
@@ -477,6 +483,8 @@ class SweepResults:
         out.server_rejected = self.server_rejected[index]
         out.server_expired = self.server_expired[index]
         out.late = self.late[index]
+        out.server_throttled = self.server_throttled[index]
+        out.lb_throttled = self.lb_throttled[index]
         out.streams = g(self.streams)
         out.band_count, out.band_sum, out.band_sumsq = self.band_count, self.band_sum, self.band_sumsq
         out.lat_window_s, out.lat_hist, out.lat_sum_hi, out.lat_sum_lo = (self.lat_window_s, self.lat_hist,
@@ -679,6 +687,8 @@ class SweepResults:
         out.server_rejected = np.concatenate([p.server_rejected for p in parts])
         out.server_expired = np.concatenate([p.server_expired for p in parts])
         out.late = np.concatenate([p.late for p in parts])
+        out.server_throttled = np.concatenate([p.server_throttled for p in parts])
+        out.lb_throttled = np.concatenate([p.lb_throttled for p in parts])
         if all(p.streams is not None for p in parts):
             out.streams = np.concatenate([p.streams for p in parts])
         if all(p.band_count is not None for p in parts):      # integer sums over disjoint replicas: they add exactly

@@ -38,7 +38,7 @@
 extern "C" {
 #endif
 
-#define AF_ABI_VERSION 11
+#define AF_ABI_VERSION 12
 
 typedef enum AfStatus {
     AF_OK = 0,
@@ -84,6 +84,10 @@ typedef struct AfServer {        /* schemas/topology/nodes.py:52-104 */
                                   * (0 = no limit; see AF_FIELD_SERVER_MAX_IN_SERVICE) */
     double deadline;             /* request deadline in seconds from creation      *
                                   * (0 = none; see AF_FIELD_SERVER_DEADLINE)       */
+    double rate_limit;           /* token-bucket rate in requests per second       *
+                                  * (0 = none; see AF_FIELD_SERVER_RATE)           */
+    int32_t burst;               /* the bucket's size (0 reads as 1)               */
+    int32_t reserved;            /* 0                                              */
 } AfServer;
 
 typedef struct AfEndpoint {      /* schemas/topology/endpoint.py:92-102 */
@@ -143,6 +147,10 @@ typedef struct AfScenario {
     const AfOutageMark* outage_marks;
     double client_timeout;       /* the client counts a completion later than this  *
                                   * as late (0 = none; AF_FIELD_CLIENT_TIMEOUT)     */
+    double lb_rate_limit;        /* the load balancer's token-bucket rate in        *
+                                  * requests per second (0 = none; AF_FIELD_LB_RATE) */
+    int32_t lb_burst;            /* its bucket's size (0 reads as 1)                */
+    int32_t reserved2;           /* 0                                               */
 } AfScenario;
 
 /* Per-replica overrides of scenario fields: the Monte-Carlo sweep
@@ -158,7 +166,11 @@ enum {
     AF_FIELD_SERVER_MAX_IN_SERVICE = 13,  /* index = server; an admission limit, 0 = none (AfServer.max_in_service) */
     AF_FIELD_SERVER_DEADLINE = 14,  /* index = server; a request deadline in seconds, 0 = none (AfServer.deadline) */
     AF_FIELD_CLIENT_TIMEOUT = 15,   /* index 0; the client's timeout in seconds, 0 = none (AfScenario.client_timeout) */
-    AF_FIELD_COUNT = 16
+    AF_FIELD_SERVER_RATE = 16,      /* index = server; a rate limit in requests per second, 0 = none (AfServer.rate_limit) */
+    AF_FIELD_SERVER_BURST = 17,     /* index = server; its burst, an integer >= 1 (AfServer.burst)                 */
+    AF_FIELD_LB_RATE = 18,          /* index 0; the load balancer's rate limit, 0 = none (AfScenario.lb_rate_limit) */
+    AF_FIELD_LB_BURST = 19,         /* index 0; its burst, an integer >= 1 (AfScenario.lb_burst)                   */
+    AF_FIELD_COUNT = 20
 };
 /* Load-balancer rows (DESIGN.md §3.11).  A replica whose row sets AF_FIELD_LB_COVERED of position k to 0 runs without
  * the LB edge lb_edges[k]: its round-robin order is lb_edges with the uncovered edges left out; the server and its other
@@ -184,6 +196,18 @@ enum {
  * The client timeout T > 0 (AfScenario.client_timeout or AF_FIELD_CLIENT_TIMEOUT) counts a completion with
  * now - t0 > T in af_fetch_late; the completion counts everywhere else as before.  Neither draws a random number.
  * af_scenario_upload and af_sweep_upload refuse negative, NaN and infinite values (the latter naming the row). */
+/* Rate limits (DESIGN.md §3.14).  A site -- a server, or the load balancer -- with a rate r > 0 requests per second
+ * (AfServer.rate_limit / AfScenario.lb_rate_limit, or the replica's AF_FIELD_SERVER_RATE / AF_FIELD_LB_RATE value) and
+ * a burst B >= 1 runs a GCRA token bucket: one f64 `tat` per site, 0 at the start.  Where the site's process takes a
+ * request from its inbox at `now`, with tau = 1/r and L = (B - 1) * tau (each correctly rounded, no FMA):
+ *     if (tat - now > L) the request is throttled; else tat = max(tat, now) + tau.
+ * A server checks right after its dispatcher takes the request, before the admission limit: a request it throttles is
+ * gone as a shed one is (no hop, no endpoint, no handler; its in-edge counts it as sent).  The load balancer checks after
+ * it takes the request and records its hop, before the pick: a request it throttles moves no round-robin order and no
+ * connection count.  af_fetch_throttled counts them.  No random number is drawn.  A burst of 0 in the scenario reads as
+ * 1.  af_scenario_upload refuses a negative, NaN or infinite rate, a negative burst and an LB rate without a load
+ * balancer; af_sweep_upload refuses a rate that is not finite and >= 0, a burst that is not an integer in [1, 2^31)
+ * (naming the row), an index out of range and the LB fields on a scenario without a load balancer. */
 typedef struct AfSweepColumn { int32_t field; int32_t index; } AfSweepColumn;
 typedef struct AfSweep {
     int32_t n_columns;
@@ -314,6 +338,9 @@ int af_fetch_server_rejected(af_engine* e, uint32_t* out, uint64_t n);
  * (all 0 when the run had no deadline and no timeout) */
 int af_fetch_server_expired(af_engine* e, uint32_t* out, uint64_t n);
 int af_fetch_late(af_engine* e, uint32_t* out, uint64_t n);
+/* requests each site throttled at its rate limit: [n][n_servers + 1], column n_servers the load balancer (all 0 when
+ * the run had no rate limit) */
+int af_fetch_throttled(af_engine* e, uint32_t* out, uint64_t n);
 int af_fetch_throughput(af_engine* e, uint32_t* out, uint64_t n);   /* [n][horizon_s]    */
 /* sampled-metric aggregates over ticks: per replica, per series j:
  *   j <  3*n_servers : server j/3, metric j%3 in {ready_queue_len, event_loop_io_sleep, ram_in_use}
